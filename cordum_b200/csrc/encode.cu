@@ -70,12 +70,14 @@ __device__ uint64_t hash_str(Str s) {
   h = mix(a ^ 0x8EBC6AF09C88C6E3ull, b ^ h);
   return h | 1;
 }
-// "a \0 b" hashed as one string without building it (host: StrTable::find_pair)
+// the pair key of host.hpp StrTable::pair_key (len(a) as 4 little-endian bytes, a, b), built in `scratch`; returns its
+// hash, and the key is Str{scratch, 4 + a.n + b.n}
 __device__ uint64_t hash_pair(Str a, Str b, uint8_t* scratch) {
-  for (uint32_t i = 0; i < a.n; ++i) scratch[i] = a.p[i];
-  scratch[a.n] = 0;
-  for (uint32_t i = 0; i < b.n; ++i) scratch[a.n + 1 + i] = b.p[i];
-  return hash_str<false>(Str{scratch, a.n + 1 + b.n});
+#pragma unroll
+  for (int i = 0; i < 4; ++i) scratch[i] = (uint8_t)(a.n >> (8 * i));
+  for (uint32_t i = 0; i < a.n; ++i) scratch[4 + i] = a.p[i];
+  for (uint32_t i = 0; i < b.n; ++i) scratch[4 + a.n + i] = b.p[i];
+  return hash_str<false>(Str{scratch, 4 + a.n + b.n});
 }
 
 __device__ __forceinline__ uint8_t lower1(uint8_t c) { return (c >= 'A' && c <= 'Z') ? (uint8_t)(c + 32) : c; }
@@ -291,12 +293,12 @@ __global__ void __launch_bounds__(128) encode_job_kernel(EncodeParams P) {
     bool shadowed = false;   // map semantics: a later entry with the same key wins
     for (uint32_t k2 = k + 1; k2 < lb && !shadowed; ++k2) shadowed = str_eq(span_of(A, P.label_keys, k2), key);
     if (shadowed) continue;
-    if (key.n + val.n > 512) { bad = true; continue; }   // the pair probes build "key \0 value" in a local buffer
+    if (key.n + val.n > 512) { bad = true; continue; }   // the pair probes build the 4 + key + value byte pair key in scratch
     // rule label pairs: labels.get(k,"") == v
     const uint32_t ki = find_exact(E, DD_LABEL_KEY, key, kMiss);
     if (ki != kMiss) {
       const uint64_t keymask = __ldg(E.label_keymask + ki);
-      const uint32_t bit = dict_find<false>(E, DD_LABEL_PAIR, Str{scratch, key.n + 1 + val.n}, hash_pair(key, val, scratch), kMiss);
+      const uint32_t bit = dict_find<false>(E, DD_LABEL_PAIR, Str{scratch, 4 + key.n + val.n}, hash_pair(key, val, scratch), kMiss);
       lab = (lab & ~keymask) | (bit < 64 ? 1ull << bit : 0ull);
     }
     const int mk = mcp_key(key);
@@ -312,7 +314,7 @@ __global__ void __launch_bounds__(128) encode_job_kernel(EncodeParams P) {
     if (!(placement_skips(key) || cordum_prefix)) {
       uint32_t bit;
       if (val.n) {
-        bit = dict_find<false>(E, DD_PLACE_PAIR, Str{scratch, key.n + 1 + val.n}, hash_pair(key, val, scratch), kMiss);
+        bit = dict_find<false>(E, DD_PLACE_PAIR, Str{scratch, 4 + key.n + val.n}, hash_pair(key, val, scratch), kMiss);
         if (bit == kMiss) flags |= JF_PLACE_UNSAT;
       } else {
         bit = find_exact(E, DD_PLACE_KEY, key, kMiss);

@@ -1266,7 +1266,7 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
     for (auto& kv : store[p.slot].labels) {
       if (place_key.find(kv.first, kMiss) == kMiss) place_key.put(kv.first, nbits++);
       if (!kv.second.empty()) {
-        std::string pk = kv.first; pk.push_back('\0'); pk += kv.second;
+        const std::string pk = StrTable::pair_key(kv.first, kv.second);
         if (place_pair.find(pk, kMiss) == kMiss) place_pair.put(pk, nbits++);
       }
     }
@@ -1325,10 +1325,7 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
         const std::string* val = nullptr;
         for (auto& kv : labels) if (kv.first == k.first) val = &kv.second;
         if (!val || val->empty()) setb(k.second);   // labels[k] == "" (matchesLabels, :169-171)
-        else {
-          std::string pk = k.first; pk.push_back('\0'); pk += *val;
-          setb(place_pair_.find(pk, 0));
-        }
+        else setb(place_pair_.find_pair(k.first, *val, 0));
       }
     }
     t.pos_label_lo[i] = m[0]; t.pos_label_hi[i] = m[1];
@@ -1848,7 +1845,7 @@ void Host::export_dicts(std::vector<uint8_t>& blob, EncodeTables& et) const {
                                     &d_risk_.table, &d_req_.table, &d_mcp_[0].table, &d_mcp_[1].table, &d_mcp_[2].table,
                                     &d_mcp_[3].table, &label_key_, nullptr, &place_pair_, &place_key_, &d_pool_.table,
                                     &worker_slot_, &effcfg_ids_};
-  StrTable label_pair;   // "key \0 value" -> bit, for the rule label pairs (host keeps them as per-key lists)
+  StrTable label_pair;   // StrTable::pair_key(key, value) -> bit, for the rule label pairs (host keeps them as per-key lists)
   std::vector<uint64_t> keymask(std::max<size_t>(label_key_pairs_.size(), 1), 0);
   for (size_t ki = 0; ki < label_key_pairs_.size(); ++ki)
     for (auto& pv : label_key_pairs_[ki])
@@ -1859,7 +1856,7 @@ void Host::export_dicts(std::vector<uint8_t>& blob, EncodeTables& et) const {
       uint32_t ki = label_key_.find(kv.first, kMiss);
       if (ki == kMiss) continue;
       for (auto& pv : label_key_pairs_[ki])
-        if (pv.first == kv.second && pv.second < 64) { std::string k = kv.first; k.push_back('\0'); k += kv.second; label_pair.put(k, pv.second); }
+        if (pv.first == kv.second && pv.second < 64) label_pair.put(StrTable::pair_key(kv.first, kv.second), pv.second);
     }
   tabs[DD_LABEL_PAIR] = &label_pair;
   for (int i = 0; i < DD_COUNT; ++i) tabs[i]->export_to(blob, et.dict[i]);

@@ -98,12 +98,24 @@ class StrTable {
       }
     }
   }
-  // key = a '\0' b, without building it
+  // a label pair as one key: len(a) as 4 little-endian bytes, a, b.  A separator byte would not do: keys and values may
+  // hold any byte, NUL included, and "a\0b" = "c" must not meet "a" = "b\0c".  encode.cu hash_pair builds the same bytes.
+  static void put_pair(char* out, sv a, sv b) {
+    const uint32_t n = (uint32_t)a.size();
+    const char len[4] = {char(n), char(n >> 8), char(n >> 16), char(n >> 24)};
+    std::memcpy(out, len, 4); std::memcpy(out + 4, a.data(), a.size()); std::memcpy(out + 4 + a.size(), b.data(), b.size());
+  }
+  static std::string pair_key(sv a, sv b) {
+    std::string k(4 + a.size() + b.size(), '\0');
+    put_pair(k.data(), a, b);
+    return k;
+  }
+  // find(pair_key(a, b)), without building it on the heap
   uint32_t find_pair(sv a, sv b, uint32_t miss) const {
-    char small[256];
-    const size_t n = a.size() + 1 + b.size();
-    if (n > sizeof small) { std::string big(a); big.push_back('\0'); big.append(b); return find(big, miss); }
-    std::memcpy(small, a.data(), a.size()); small[a.size()] = 0; std::memcpy(small + a.size() + 1, b.data(), b.size());
+    char small[260];
+    const size_t n = 4 + a.size() + b.size();
+    if (n > sizeof small) return find(pair_key(a, b), miss);
+    put_pair(small, a, b);
     return find(sv(small, n), miss);
   }
   bool contains(sv key) const { return find(key, 0xFFFFFFFEu) != 0xFFFFFFFEu; }
@@ -359,6 +371,9 @@ class Host {
   const std::string& topic_raw(uint32_t topic_id) const { return (*topic_store_)[topic_id]; }
   std::shared_ptr<const std::vector<std::string>> topic_text() const { return topic_store_; }
   uint64_t dict_resets() const { return dict_resets_; }
+  // the encoders' sort key of a job: topic id * tenant_classes() + tenant_class()[tenant dictionary id]
+  uint32_t tenant_classes() const { return std::max<uint32_t>(1, tenant_classes_); }
+  const std::vector<uint8_t>& tenant_class() const { return tenant_class_; }
   uint32_t wide_words() const { return WIDE_WORDS(t_.wide); }
   uint64_t policy_generation() const { return text_gen_.load(std::memory_order_acquire); }
   std::string mcp_value_string(int field, uint32_t id) const;
@@ -433,7 +448,7 @@ class Host {
   std::atomic<uint64_t> text_gen_{0};                   // generation of text_.back(), readable without the lock
   void publish_text();
   StrTable worker_slot_;      // worker_id -> slot (last wins)
-  StrTable place_pair_;       // key '\0' value -> bit   (value non-empty)
+  StrTable place_pair_;       // StrTable::pair_key(key, value) -> bit   (value non-empty)
   StrTable place_key_;        // key -> bit E_k ("labels non-empty and k absent-or-empty")
   uint32_t place_any_bit_ = 0; // bit "worker has >= 1 label"
   uint32_t place_bits_ = 0;

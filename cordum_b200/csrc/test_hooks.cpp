@@ -83,6 +83,7 @@ int32_t cordum_test_host_table(void* h, const char* name, const void** ptr, uint
   VEC("slot_pos", t.slot_pos) VEC("rank_slot", t.rank_slot) VEC("pos_label_lo", t.pos_label_lo)
   VEC("pos_label_hi", t.pos_label_hi) VEC("loads", t.loads)
   VEC("chunk_pool", t.chunk_pool) VEC("pool_chunk0", t.pool_chunk0) VEC("merge_list", t.merge_list)
+  VEC("tenant_class", ((Host*)h)->tenant_class())
 #undef VEC
   t_err = "unknown table " + n;
   return -1;
@@ -107,6 +108,7 @@ uint64_t cordum_test_host_scalar(void* h, const char* name) {
   if (n == "n_slots") return t.n_slots;
   if (n == "n_topics") return t.row_topic.n_rows;
   if (n == "dict_resets") return ((Host*)h)->dict_resets();
+  if (n == "tenant_classes") return ((Host*)h)->tenant_classes();
   if (n == "xw_risk") return t.wide.xw_risk;
   if (n == "xw_req") return t.wide.xw_req;
   if (n == "xw_lab") return t.wide.xw_lab;

@@ -10,6 +10,9 @@ Python-level shapes mirror the CAP v2 messages the reference reads on this path
                      "capability": str, "risk_tags": [str], "requires": [str],
                      "pack_id": str},
      "effective_config": bytes|str, "approved": bool}
+    "labels" may also be a list of (key, value) pairs, laid out in that order, repeated keys
+    included (the encoders give a repeated key its last value, as a map decoded from the
+    wire would hold it)
   worker (Heartbeat fields, snapshot.go:20-28):
     {"worker_id": str, "pool": str, "active_jobs": int, "max_parallel_jobs": int,
      "cpu_load": float, "gpu_utilization": float, "labels": {str: str}}
@@ -236,7 +239,8 @@ class EnvelopeBatch:
                     risk.append(ar.add(t))
                 for t in meta.get("requires") or []:
                     req.append(ar.add(t))
-            for k, v in (job.get("labels") or {}).items():
+            labels = job.get("labels") or {}
+            for k, v in (labels.items() if isinstance(labels, dict) else labels):
                 lk.append(ar.add(k))
                 lv.append(ar.add(v))
             approved[j] = 1 if job.get("approved") else 0

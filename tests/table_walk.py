@@ -39,9 +39,10 @@ TABLES = {
     "pos_label_lo": np.uint64, "pos_label_hi": np.uint64, "loads": wire.LOAD_DTYPE,
     "chunk_pool": np.uint32, "pool_chunk0": np.uint32, "merge_list": np.uint32,
     "rule_need_x": np.uint64, "pool_req_x": np.uint64, "req_blank_x": np.uint64, "pos_label_x": np.uint64,
+    "tenant_class": np.uint8,
 }
 SCALARS = ["n_rules", "n_seg", "sum_group", "sum_use", "n_chunks", "n_merge", "merge_smem", "row_words", "mcp_stride", "topic_stride", "n_effcfg", "req_blank_mask", "n_pools",
-           "n_pos", "n_slots", "n_topics", "xw_risk", "xw_req", "xw_lab", "xw_place", "place_bits", "dict_resets"]
+           "n_pos", "n_slots", "n_topics", "xw_risk", "xw_req", "xw_lab", "xw_place", "place_bits", "dict_resets", "tenant_classes"]
 
 
 def _align16(x):

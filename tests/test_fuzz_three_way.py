@@ -7,6 +7,7 @@ MCP aliases, effective configs, legacy tenant rules, ties, overloaded workers):
 
 The reference's own tests pin none of these interactions (SURVEY.md §8c, last row); agreement of two restatements
 written from the cited lines, plus the product's table compiler + encoder, is what stands in for them.  CPU only."""
+import contextlib
 import json
 import os
 import random
@@ -50,6 +51,43 @@ MCP_VALS += ["\u2003srv\u2003", "s\u0280v"]
 PATTERNS += ["job.\u00e9*", "\u00a0job.sre.*\u00a0", "job.[\u00e0-\u00ff]*.*", "job.?\u00e9.*"]
 PACKS += ["\u00e9t\u00e9"]
 DECISIONS = ["allow", "deny", "require_approval", "throttle", "allow_with_constraints", "permit", "block", "REQUIRE-HUMAN", ""]
+
+
+
+def _ascii_vocabulary():
+    """Module globals for ascii_case: the ASCII entries of the vocabularies above plus awkward ASCII of their own - control
+    bytes TrimSpace keeps (NUL, 0x1C-0x1F, DEL), \\v \\f \\r\\n padding, mixed-case values longer than 16 and than 160 bytes
+    (every length class of the folding hash), and NUL inside label keys and values, where "a\\0b" = "c" and "a" = "b\\0c"
+    are different pairs.  No string needs Unicode tables, so the device encoder keeps every batch (encode.cu)."""
+    asc = lambda xs: [x for x in xs if x.isascii()]   # noqa: E731
+    long_t, long_c = "Tenant-Of-" + "MiXeD" * 33, "Cap.Of-Mixed-Case-" + "Ab" * 80   # 175 and 178 bytes
+    return dict(
+        TENANTS=asc(TENANTS) + ["\vt1\f", "t1\r\n", "\x1ct1", "t1\x7f", "\x00t1", "T1\x1f", "Tenant-Mixed-Case", "tenant-mixed-case\r\n",
+                                long_t, " " + long_t.lower()],
+        PACKS=asc(PACKS) + ["Pack-Of-Mixed-Case", "\x1e"],
+        CAPS=asc(CAPS) + ["\fcap.read\v", "cap.read\x00", "CAP.Of-Mixed-Case-Xy", "cap.of-mixed-case-xy\r\n", long_c, long_c.upper()],
+        RISKS=asc(RISKS) + ["\vwrite", "WRITE\r\n", "write\x1d", "Risk-Of-Mixed-Case", "risk-of-mixed-case\f", "SeCrEtS"],
+        REQS=asc(REQS) + ["\vgit\f", "Git\r\n", "git\x7f", "Requires-Mixed-Case", " requires-mixed-case"],
+        LKEYS=asc(LKEYS) + ["a", "a\x00b", "Env"],
+        LVALS=asc(LVALS) + ["b\x00c", "c", "\x00", "PROD", " prod"],
+        ACTORS=asc(ACTORS) + ["\x1falice", "ALICE\r\n", "Actor-Of-Mixed-Case-" + "Q" * 150],
+        MCP_VALS=asc(MCP_VALS) + ["\vsrv\f", "Srv\r\n", "\x1fsrv", "srv\x00", "Server-Of-Mixed-Case", "server-of-mixed-case\v"],
+        PATTERNS=asc(PATTERNS) + ["\vjob.sre.*", "job.db.*\r\n", "job.\x00*"],
+    )
+
+
+@contextlib.contextmanager
+def vocabulary(v):
+    """The generators read the module's vocabulary globals: swap them for `v` inside the block."""
+    me = sys.modules[__name__]
+    old = {k: getattr(me, k) for k in v}
+    for k, x in v.items():
+        setattr(me, k, x)
+    try:
+        yield
+    finally:
+        for k, x in old.items():
+            setattr(me, k, x)
 
 
 def pick(rng, xs, lo=0, hi=2):
@@ -186,6 +224,8 @@ def py_records(policy, routing, workers, jobs):
     live = list({w["worker_id"]: w for w in workers}.values())   # registry semantics: the latest heartbeat wins
     out = []
     for job in jobs:
+        if isinstance(job.get("labels"), list):   # repeated keys: the map the reference decodes holds the last value
+            job = dict(job, labels=dict(job["labels"]))
         r = py_oracle.process_job(policy, routing, live, job)
         rt = r["route"]
         out.append((wire.DEC_NAMES.index(r["decision"]), wire.DEC_NAMES.index(r["sched_decision"]), r["rule_idx"],
@@ -273,6 +313,43 @@ def life_cycle(seed, steps=6):
         yield kind, payload, [make_job(rng, workers) for _ in range(30)]
 
 
+def ascii_case(seed, max_rules):
+    """fuzz_case with the ASCII-only awkward vocabulary of _ascii_vocabulary."""
+    with vocabulary(_ascii_vocabulary()):
+        return fuzz_case(seed, max_rules)
+
+
+def ascii_life_cycle(seed):
+    """The steps of life_cycle(seed), drawn from the ASCII-only vocabulary."""
+    with vocabulary(_ascii_vocabulary()):
+        return list(life_cycle(seed))
+
+
+DUP_KEYS = ["mcp.server", "mcp_server", "mcpServer", "mcp.tool", "mcp_tool", "mcpTool", "mcp.resource", "mcp_resource", "mcpResource",
+            "mcp.action", "mcp_action", "mcpAction", "secrets_present", "preferred_pool", "preferred_worker_id"]
+
+
+def dup_case(seed):
+    """ascii_case(seed, 12) with repeated label keys spliced into most jobs: labels become a list of (key, value) pairs in
+    which some keys - ordinary and rule label keys, placement keys, every MCP alias, secrets_present and the routing
+    hints - occur two or three times with different values.  Only the last occurrence counts."""
+    policy, routing, workers, jobs = ascii_case(seed, 12)
+    voc = _ascii_vocabulary()
+    rng = random.Random(21000 + seed)
+    values = {"secrets_present": ["true", "TRUE", "1", "yes", "no", " true ", ""], "preferred_pool": POOLS + ["nope", ""],
+              "preferred_worker_id": [w["worker_id"] for w in workers] + ["ghost", ""]}
+    for j in jobs:
+        if rng.random() < 0.2:
+            continue
+        items = list((j.get("labels") or {}).items())
+        for k in rng.sample(voc["LKEYS"] + DUP_KEYS, rng.randint(1, 4)) + [k for k, _ in items if rng.random() < 0.5]:
+            vals = values.get(k, voc["MCP_VALS"] if k.startswith("mcp") else voc["LVALS"])
+            for _ in range(rng.randint(2, 3)):
+                items.insert(rng.randint(0, len(items)), (k, rng.choice(vals)))
+        j["labels"] = items
+    return policy, routing, workers, jobs
+
+
 def sparse_summary_case():
     """(policy, routing, workers, jobs) whose risk-tag, capability and pack rows are sparse: 96 tags (32 of them beyond the
     record's 64-bit mask), each owning one block of 32 consecutive rules, so a tag's row - and its summary - covers one
@@ -327,6 +404,10 @@ def test_three_implementations_agree(seed, max_rules, sum_use, monkeypatch):
     the walk skips word groups by whichever summaries the knob names (the table compiler reads it on every rebuild)."""
     force_sum_use(monkeypatch, sum_use)
     policy, routing, workers, jobs = fuzz_case(seed, max_rules)
+    agree_three_ways(seed, policy, routing, workers, jobs, sum_use)
+
+
+def agree_three_ways(seed, policy, routing, workers, jobs, sum_use=None):
     env = wire.EnvelopeBatch.from_jobs(jobs)
     o = oracle_lib.Oracle(policy, routing, workers)
     h = table_walk.HostHarness(policy, routing, workers)
@@ -346,13 +427,38 @@ def test_three_implementations_agree(seed, max_rules, sum_use, monkeypatch):
     assert not bad, "seed %d C++ vs Python oracle: %s\n%s" % (seed, bad[:3], json.dumps(jobs[bad[0][0]]))
 
 
+@pytest.mark.parametrize("seed,max_rules", [(s, 12) for s in range(60)] + [(100 + s, 400) for s in range(12)])
+def test_three_implementations_agree_on_ascii_vocabulary(seed, max_rules):
+    """The ASCII-only awkward vocabulary (_ascii_vocabulary): the inputs the device encoder keeps to itself, checked against
+    both oracles here so that the GPU tests can take the host encoder as their reference."""
+    agree_three_ways(seed, *ascii_case(seed, max_rules))
+
+
+@pytest.mark.parametrize("seed", range(60))
+def test_three_implementations_agree_on_repeated_label_keys(seed):
+    """Labels with repeated keys (dup_case): the last value wins for rule label pairs, placement, every MCP alias,
+    secrets_present and the routing hints."""
+    policy, routing, workers, jobs = dup_case(seed)
+    assert sum(len(j.get("labels") or []) > len(dict(j.get("labels") or [])) for j in jobs) >= len(jobs) // 2
+    agree_three_ways(seed, policy, routing, workers, jobs)
+
+
 @pytest.mark.parametrize("seed", range(30))
 def test_reloads_and_heartbeats_keep_agreeing(seed):
     """The same engine-side objects across a life cycle: heartbeat deltas (loads by slot), a worker-registry reload, a
     routing reload and a policy reload, each followed by a re-evaluation of freshly encoded jobs - dictionaries are
     rebuilt, ids are reassigned and the tables must still agree with an oracle that went through the same calls."""
+    check_life_cycle(seed, life_cycle(seed))
+
+
+@pytest.mark.parametrize("seed", range(30))
+def test_reloads_and_heartbeats_keep_agreeing_on_ascii_vocabulary(seed):
+    check_life_cycle(seed, ascii_life_cycle(seed))
+
+
+def check_life_cycle(seed, steps):
     o = h = None
-    for step, (kind, payload, jobs) in enumerate(life_cycle(seed)):
+    for step, (kind, payload, jobs) in enumerate(steps):
         if kind == "load":
             o, h = oracle_lib.Oracle(*payload), table_walk.HostHarness(*payload)
         elif kind == "heartbeat" and payload is not None:

@@ -54,6 +54,8 @@ def eng(request):
 
     engine.Batch.default_device_encode = request.param == "device-encode"
     e = engine.Engine(device=0)
+    # batches the device encoder was given / completed without handing them to the host (test_device_encoder_kept_batches)
+    e.device_encodes = {"tried": 0, "kept": 0} if request.param == "device-encode" else None
     yield e
     e.close()
     engine.Batch.default_device_encode = False
@@ -88,7 +90,11 @@ def compare(e, o, jobs, what, modes=MODES):
     out = {}
     try:
         for mode in modes:
+            f0 = e.host_fallbacks()
             got = b.encode(env).dispatch(mode).copy()
+            if getattr(e, "device_encodes", None) is not None:
+                e.device_encodes["tried"] += 1
+                e.device_encodes["kept"] += e.host_fallbacks() == f0
             assert_same(got, o.eval(env, mode, threads=usable_cores()), "%s, %s" % (what, MODE_NAMES[mode]), listed)
             out[mode] = got
     finally:
@@ -570,3 +576,15 @@ def test_multi_tile_grids_and_kernel_instances(minb, route_minb):
     print(r.stdout, r.stderr)
     assert r.returncode == 0, "MINB=%d ROUTE_MINB=%d: exit %d\n%s\n%s" % (minb, route_minb, r.returncode, r.stdout, r.stderr)
     assert r.stdout.count("records compared") == 3
+
+
+def test_device_encoder_kept_batches(eng):
+    """The device-encode half of this module means something only if batches completed on the device: a batch that falls
+    back is re-encoded by the host encoder, and its records then say nothing about encode.cu.  Runs after the other tests
+    of its encoder (the module fixture groups them)."""
+    if eng.device_encodes is None:
+        pytest.skip("host encoder")
+    if eng.device_encodes["tried"] == 0:
+        pytest.skip("no device-encoded batch ran in this session")
+    print("device-encoded batches: %d of %d completed on the device" % (eng.device_encodes["kept"], eng.device_encodes["tried"]))
+    assert eng.device_encodes["kept"] > 0

@@ -351,3 +351,38 @@ def test_dynamic_dictionaries_start_a_new_generation_when_full():
     with pytest.raises(RuntimeError, match="effective configs"):
         h.evaluate([{"topic": "job.keep.a", "effective_config": ('{"safety":{"denied_topics":["x%d"]}}' % i).encode()} for i in range(9)])
     o.close()
+
+
+# Label pairs whose keys or values hold NUL.  Both are valid (a protobuf string, a Go map key), so "a\0b" = "c" and
+# "a" = "b\0c" are different pairs; a pair key that joins key and value with a separator byte makes them one.
+# (name, policy, routing, workers, jobs)
+NUL_ROUTING = {"topics": {"job.x": ["p"]}, "pools": {"p": {}}}
+NUL_PAIR_CASES = [
+    ("job-key-holds-nul", None, NUL_ROUTING,
+     [kats.hb("w0", "p", 0, 10.0, 0.0, 0, {"a": "b\0c"}), kats.hb("w1", "p", 0, 50.0, 0.0, 0, {"z": "1"})],
+     [{"topic": "job.x", "labels": {"a\0b": "c"}}, {"topic": "job.x", "labels": {"a": "b\0c"}}, {"topic": "job.x", "labels": {"a": "b"}}]),
+    ("job-value-holds-nul", None, NUL_ROUTING,
+     [kats.hb("w0", "p", 0, 10.0, 0.0, 0, {"a\0b": "c"}), kats.hb("w1", "p", 0, 50.0, 0.0, 0, {"z": "1"})],
+     [{"topic": "job.x", "labels": {"a": "b\0c"}}, {"topic": "job.x", "labels": {"a\0b": "c"}}, {"topic": "job.x", "labels": {"a\0b": ""}}]),
+    ("colliding-workers", None, NUL_ROUTING,   # the less loaded worker holds the other pair of the collision
+     [kats.hb("w0", "p", 0, 10.0, 0.0, 0, {"a": "b\0c"}), kats.hb("w1", "p", 0, 50.0, 0.0, 0, {"a\0b": "c"}),
+      kats.hb("w2", "p", 0, 5.0, 0.0, 0, {"a\0": "\0b\0c"})],
+     [{"topic": "job.x", "labels": {"a\0b": "c"}}, {"topic": "job.x", "labels": {"a": "b\0c"}}, {"topic": "job.x", "labels": {"a\0": "\0b\0c"}},
+      {"topic": "job.x", "labels": {"a\0b\0": "c"}}]),
+    ("rule-labels", {"default_tenant": "default", "rules": [
+        {"id": "r0", "decision": "deny", "reason": "a is b-nul-c", "match": {"labels": {"a": "b\0c"}}},
+        {"id": "r1", "decision": "require_approval", "reason": "a-nul-b is x", "match": {"labels": {"a\0b": "x"}}}]},
+     NUL_ROUTING, [kats.hb("w0", "p")],
+     [{"topic": "job.x", "labels": {"a\0b": "c"}}, {"topic": "job.x", "labels": {"a\0b": "x"}}, {"topic": "job.x", "labels": {"a": "b\0c"}},
+      {"topic": "job.x", "labels": {"a": "b\0c", "a\0b": "x"}}, {"topic": "job.x", "labels": {"a": "b"}}]),
+]
+
+
+@pytest.mark.parametrize("name,policy,routing,workers,jobs", NUL_PAIR_CASES, ids=[c[0] for c in NUL_PAIR_CASES])
+def test_label_pairs_with_nul_bytes_do_not_collide(name, policy, routing, workers, jobs):
+    h = table_walk.HostHarness(policy, routing, workers)
+    o = oracle_lib.Oracle(policy, routing, workers)
+    for mode in (wire.MODE_POLICY_AND_ROUTE, wire.MODE_POLICY_ONLY, wire.MODE_ROUTE_ONLY):
+        assert_same(h.evaluate(jobs, mode), o.eval(jobs, mode), "%s mode %d" % (name, mode))
+    h.close()
+    o.close()
