@@ -29,9 +29,13 @@ using cordum::sv;
 namespace {
 thread_local std::string g_err;
 
-struct DevBuf {
+struct DevBuf {   // a device allocation that grows on demand and is freed with its owner
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
   cudaError_t upload(const void* src, size_t bytes, cudaStream_t s) {
     if (bytes > cap) {
       if (p) cudaFree(p);
@@ -52,7 +56,6 @@ struct DevBuf {
     cap = e == cudaSuccess ? bytes : 0;
     return e;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
 // record slab for n jobs: n JobRec (64 B), then n RouteRec (32 B) - one contiguous H2D copy of 96 B per job
@@ -93,9 +96,12 @@ struct cordum_engine {
   uint64_t v_dict = ~0ull;
   std::vector<cordum_envelopes*> env_sets;   // pinned envelope staging sets handed out by cordum_envelopes_alloc
   uint64_t tables_gen = 0;       // bumps whenever a device table pointer or scalar may have changed (captured graphs bake them in)
+  // Pinned staging of this rank's heartbeat slice (+ the epoch word behind it), one per gather-buffer parity.  The ingest
+  // graphs and the ticks share it: leave_tick_mode drains the tick streams before any ingest, and cordum_tick_async
+  // synchronises the device when it enters tick mode, so the two never have a copy out of it in flight at once.
+  Load16* stage[2] = {nullptr, nullptr};
+  size_t stage_cap = 0;
   // ---- cordum_workers_ingest as one graph launch (world = 1, or the peer exchange): H2D -> [peer gather] -> chunk -> merge
-  Load16* ing_stage[2] = {nullptr, nullptr};   // pinned staging of the caller's slice (+ the epoch word behind it)
-  size_t ing_cap = 0;
   std::map<std::tuple<int, int, uint64_t>, cudaGraphExec_t> ing_graphs;   // (target set, buffer parity, tables generation)
   // ---- scheduler ticks (cordum_tick_async): one CUDA graph launch per tick
   struct Tick {
@@ -107,8 +113,6 @@ struct cordum_engine {
     cudaEvent_t refreshed[2] = {nullptr, nullptr};         // recorded inside graph k at the end of its heartbeat branch: the
                                                            // heartbeat branch of tick k+1 starts behind it (the epochs stay ordered)
     cudaEvent_t ev_join = nullptr;
-    Load16* h_slice[2] = {nullptr, nullptr};               // pinned staging of this rank's heartbeat slice
-    size_t h_cap = 0;
     cordum_batch* prev = nullptr;                          // its policy ran in the previous tick; its route is due
     uint64_t n = 0;                                        // ticks so far
     bool active = false;                                   // ticks have been issued since the last plain dispatch / ingest
@@ -131,7 +135,6 @@ struct cordum_engine {
     cudaEvent_t ready = nullptr, loads_read = nullptr;   // refresh complete / load table consumed by the refresh
   } ds[kSets];
   int cur = 0;                   // set holding the latest refresh
-  bool host_loads = true;        // the next refresh takes the loads from the host tables
   uint64_t v_policy = ~0ull, v_topic = ~0ull, v_mcp = ~0ull, v_routing = ~0ull, v_workers = ~0ull, v_loads = ~0ull;
   std::vector<cordum_batch*> batches;   // live batches (guarded by mu): K2 must wait for their kernels
   bool pools_dirty = true;       // K2 must run before the next dispatch
@@ -195,8 +198,13 @@ void device_records(const cordum_batch* b, JobRecords& r) {
   r.wide = b->wide_words ? b->d_wide : nullptr;
 }
 
-template <class T>
-cudaError_t up(DevBuf& b, const std::vector<T>& v, cudaStream_t s) { return b.upload(v.data(), v.size() * sizeof(T), s); }
+// Uploads a host table into b and points the kernels' view (field) at it.
+template <class T, class P>
+cudaError_t put(DevBuf& b, const std::vector<T>& v, const P*& field, cudaStream_t s) {
+  cudaError_t err = b.upload(v.data(), v.size() * sizeof(T), s);
+  field = (const P*)b.p;
+  return err;
+}
 
 // Bring the device tables up to date with the host tables.  Called with host mutex held.
 int sync_tables(cordum_engine* e) {
@@ -223,101 +231,79 @@ int sync_tables(cordum_engine* e) {
         const uint32_t* row = tabs[k]->row((uint32_t)v);
         for (size_t w = 0; w < w4; ++w) std::memcpy(&wm[(w * cells + off[k] + v) * 4], row + 4 * w, 16);
       }
-    CK(up(e->b_rows, wm, s), "upload");
+    CK(put(e->b_rows, wm, d.rows, s), "upload");
     CK(cudaStreamSynchronize(s), "upload");   // wm is a local
-    d.rows = (const Row16*)e->b_rows.p; d.n_cells = cells;
+    d.n_cells = cells;
     d.off_topic = off[0]; d.off_tenant = off[1]; d.off_cap = off[2]; d.off_pack = off[3]; d.off_actor = off[4];
     d.off_combo = off[5]; d.off_risk = off[6];
     for (int f = 0; f < 4; ++f) d.off_mcp[f] = off[7 + f];
     d.n_topic = t.row_topic.n_rows;
   }
   if (t.v_policy != e->v_policy) {
-    CK(up(e->b_row_check, t.row_check.data, s), "upload");
-    CK(up(e->b_sum_tenant, t.sum_tenant, s), "upload"); CK(up(e->b_sum_cap, t.sum_cap, s), "upload");
-    CK(up(e->b_sum_pack, t.sum_pack, s), "upload"); CK(up(e->b_sum_actor, t.sum_actor, s), "upload");
-    CK(up(e->b_sum_combo, t.sum_combo, s), "upload"); CK(up(e->b_sum_risk, t.sum_risk, s), "upload");
-    CK(up(e->b_req_need, t.rule_req_need, s), "upload"); CK(up(e->b_lab_need, t.rule_lab_need, s), "upload");
-    CK(up(e->b_rule_dec, t.rule_dec, s), "upload"); CK(up(e->b_pos2rule, t.pos2rule, s), "upload");
-    d.pos2rule = (const uint32_t*)e->b_pos2rule.p;
+    CK(put(e->b_row_check, t.row_check.data, d.chk_words, s), "upload");
+    CK(put(e->b_sum_tenant, t.sum_tenant, d.sum_tenant, s), "upload"); CK(put(e->b_sum_cap, t.sum_cap, d.sum_cap, s), "upload");
+    CK(put(e->b_sum_pack, t.sum_pack, d.sum_pack, s), "upload"); CK(put(e->b_sum_actor, t.sum_actor, d.sum_actor, s), "upload");
+    CK(put(e->b_sum_combo, t.sum_combo, d.sum_combo, s), "upload"); CK(put(e->b_sum_risk, t.sum_risk, d.sum_risk, s), "upload");
+    CK(put(e->b_req_need, t.rule_req_need, d.rule_req_need, s), "upload");
+    CK(put(e->b_lab_need, t.rule_lab_need, d.rule_lab_need, s), "upload");
+    CK(put(e->b_rule_dec, t.rule_dec, d.rule_dec, s), "upload"); CK(put(e->b_pos2rule, t.pos2rule, d.pos2rule, s), "upload");
     d.n_rules = t.n_rules; d.n_seg = t.n_seg; d.row_u4 = t.n_seg * CORDUM_SEG_U4; d.sum_group = t.sum_group;
-    d.sum_tenant = (const uint64_t*)e->b_sum_tenant.p; d.sum_cap = (const uint64_t*)e->b_sum_cap.p;
-    d.sum_pack = (const uint64_t*)e->b_sum_pack.p; d.sum_actor = (const uint64_t*)e->b_sum_actor.p;
-    d.sum_combo = (const uint64_t*)e->b_sum_combo.p; d.sum_risk = (const uint64_t*)e->b_sum_risk.p;
-    d.chk_words = (const uint32_t*)e->b_row_check.p;
-    d.rule_req_need = (const uint64_t*)e->b_req_need.p; d.rule_lab_need = (const uint64_t*)e->b_lab_need.p;
-    d.rule_dec = (const uint8_t*)e->b_rule_dec.p;
-    CK(up(e->b_rule_need_x, t.rule_need_x, s), "upload");
-    d.rule_need_x = (const uint64_t*)e->b_rule_need_x.p;
+    CK(put(e->b_rule_need_x, t.rule_need_x, d.rule_need_x, s), "upload");
     e->v_policy = t.v_policy;
   }
   if (t.v_topic != e->v_topic) {
-    CK(up(e->b_sum_topic, t.sum_topic, s), "upload");
-    CK(up(e->b_eff_topic, t.eff_topic, s), "upload");
-    CK(up(e->b_topic_pool_off, t.topic_pool_off, s), "upload"); CK(up(e->b_topic_pool_cnt, t.topic_pool_cnt, s), "upload");
-    CK(up(e->b_pool_list, t.pool_list, s), "upload");
-    d.sum_topic = (const uint64_t*)e->b_sum_topic.p;
+    CK(put(e->b_sum_topic, t.sum_topic, d.sum_topic, s), "upload");
+    CK(put(e->b_eff_topic, t.eff_topic, d.eff_topic, s), "upload");
+    CK(put(e->b_topic_pool_off, t.topic_pool_off, d.topic_pool_off, s), "upload");
+    CK(put(e->b_topic_pool_cnt, t.topic_pool_cnt, d.topic_pool_cnt, s), "upload");
+    CK(put(e->b_pool_list, t.pool_list, d.pool_list, s), "upload");
     d.sum_use = t.sum_use;   // chosen against the topic rows (Host::choose_summaries)
-    d.eff_topic = (const uint8_t*)e->b_eff_topic.p; d.topic_stride = t.topic_stride;
-    d.topic_pool_off = (const uint32_t*)e->b_topic_pool_off.p; d.topic_pool_cnt = (const uint32_t*)e->b_topic_pool_cnt.p;
-    d.pool_list = (const uint32_t*)e->b_pool_list.p;
+    d.topic_stride = t.topic_stride;
     e->v_topic = t.v_topic;
   }
   if (t.v_mcp != e->v_mcp) {
-    CK(up(e->b_tenant_mcp, t.tenant_mcp, s), "upload"); CK(up(e->b_eff_mcp, t.eff_mcp, s), "upload");
-    d.tenant_mcp = (const uint8_t*)e->b_tenant_mcp.p; d.eff_mcp = (const uint8_t*)e->b_eff_mcp.p; d.mcp_stride = t.mcp_stride;
+    CK(put(e->b_tenant_mcp, t.tenant_mcp, d.tenant_mcp, s), "upload"); CK(put(e->b_eff_mcp, t.eff_mcp, d.eff_mcp, s), "upload");
+    d.mcp_stride = t.mcp_stride;
     e->v_mcp = t.v_mcp;
   }
   if (t.v_routing != e->v_routing) {
-    CK(up(e->b_pool_req_mask, t.pool_req_mask, s), "upload"); CK(up(e->b_pool_req_nonempty, t.pool_req_nonempty, s), "upload");
-    d.pool_req_mask = (const uint64_t*)e->b_pool_req_mask.p; d.pool_req_nonempty = (const uint8_t*)e->b_pool_req_nonempty.p;
+    CK(put(e->b_pool_req_mask, t.pool_req_mask, d.pool_req_mask, s), "upload");
+    CK(put(e->b_pool_req_nonempty, t.pool_req_nonempty, d.pool_req_nonempty, s), "upload");
     d.req_blank_mask = t.req_blank_mask; d.n_pools = t.n_pools;
-    CK(up(e->b_pool_req_x, t.pool_req_x, s), "upload"); CK(up(e->b_req_blank_x, t.req_blank_x, s), "upload");
-    d.pool_req_x = (const uint64_t*)e->b_pool_req_x.p; d.req_blank_x = (const uint64_t*)e->b_req_blank_x.p;
+    CK(put(e->b_pool_req_x, t.pool_req_x, d.pool_req_x, s), "upload"); CK(put(e->b_req_blank_x, t.req_blank_x, d.req_blank_x, s), "upload");
     e->v_routing = t.v_routing;
   }
   if (t.v_workers != e->v_workers) {
-    CK(up(e->b_pool_off, t.pool_off, s), "upload"); CK(up(e->b_pos_pool, t.pos_pool, s), "upload");
-    CK(up(e->b_pos_slot, t.pos_slot, s), "upload"); CK(up(e->b_pos_rank, t.pos_rank, s), "upload");
-    CK(up(e->b_slot_pos, t.slot_pos, s), "upload"); CK(up(e->b_rank_slot, t.rank_slot, s), "upload");
-    CK(up(e->b_rank_pos, t.rank_pos, s), "upload");
-    d.rank_pos = (const uint32_t*)e->b_rank_pos.p;
-    CK(up(e->b_pos_label_lo, t.pos_label_lo, s), "upload"); CK(up(e->b_pos_label_hi, t.pos_label_hi, s), "upload");
+    CK(put(e->b_pool_off, t.pool_off, d.pool_off, s), "upload"); CK(put(e->b_pos_pool, t.pos_pool, d.pos_pool, s), "upload");
+    CK(put(e->b_pos_slot, t.pos_slot, d.pos_slot, s), "upload"); CK(put(e->b_pos_rank, t.pos_rank, d.pos_rank, s), "upload");
+    CK(put(e->b_slot_pos, t.slot_pos, d.slot_pos, s), "upload"); CK(put(e->b_rank_slot, t.rank_slot, d.rank_slot, s), "upload");
+    CK(put(e->b_rank_pos, t.rank_pos, d.rank_pos, s), "upload");
+    CK(put(e->b_pos_label_lo, t.pos_label_lo, d.pos_label_lo, s), "upload");
+    CK(put(e->b_pos_label_hi, t.pos_label_hi, d.pos_label_hi, s), "upload");
+    // the derived tables of every set, sized for the new registry
+    const size_t pos = std::max<uint32_t>(t.n_pos, 1), pools = std::max<uint32_t>(t.n_pools, 1);
+    const size_t lbest = t.place_bits <= CORDUM_LBEST_MAX_BITS ? pools * t.place_bits * 16 : 0;   // 0: not built
     for (auto& D : e->ds) {
-      CK(D.pos_key.reserve((size_t)std::max<uint32_t>(t.n_pos, 1) * 8), "alloc");
-      CK(D.pool_best.reserve((size_t)std::max<uint32_t>(t.n_pools, 1) * 8), "alloc");
-      CK(D.pool_mincnt.reserve((size_t)std::max<uint32_t>(t.n_pools, 1) * 4), "alloc");
-      CK(D.skey.reserve((size_t)std::max<uint32_t>(t.n_pos, 1) * 8), "alloc");
-      CK(D.ckey.reserve((size_t)std::max<uint32_t>(t.n_pos, 1) * 8), "alloc");
-      CK(D.pool_sorted.reserve((size_t)std::max<uint32_t>(t.n_pools, 1)), "alloc");
-      CK(D.pool_nok.reserve((size_t)std::max<uint32_t>(t.n_pools, 1) * 4), "alloc");
-      CK(D.pool_done.reserve((size_t)std::max<uint32_t>(t.n_pools, 1) * 4), "alloc");
-      CK(D.lbm.reserve((size_t)std::max<uint64_t>(t.lbm_words, 1) * 4), "alloc");
-      if (t.place_bits <= CORDUM_LBEST_MAX_BITS) CK(D.lbest.reserve((size_t)std::max<uint32_t>(t.n_pools, 1) * t.place_bits * 16), "alloc");
-      CK(D.loads.reserve((size_t)std::max<uint32_t>(t.n_slots, 1) * sizeof(Load16)), "alloc");
+      const std::pair<DevBuf*, size_t> sizes[] = {
+          {&D.pos_key, pos * 8}, {&D.pool_best, pools * 8}, {&D.pool_mincnt, pools * 4}, {&D.skey, pos * 8}, {&D.ckey, pos * 8},
+          {&D.pool_sorted, pools}, {&D.pool_nok, pools * 4}, {&D.pool_done, pools * 4},
+          {&D.lbm, (size_t)std::max<uint64_t>(t.lbm_words, 1) * 4}, {&D.lbest, lbest},
+          {&D.loads, (size_t)std::max<uint32_t>(t.n_slots, 1) * sizeof(Load16)}};
+      for (const auto& [buf, bytes] : sizes) CK(buf->reserve(bytes), "alloc");
     }
-    CK(up(e->b_chunk_pool, t.chunk_pool, s), "upload"); CK(up(e->b_pool_chunk0, t.pool_chunk0, s), "upload");
-    CK(up(e->b_merge_list, t.merge_list, s), "upload");
-    d.chunk_pool = (const uint32_t*)e->b_chunk_pool.p; d.pool_chunk0 = (const uint32_t*)e->b_pool_chunk0.p;
-    d.merge_list = (const uint32_t*)e->b_merge_list.p;
+    CK(put(e->b_chunk_pool, t.chunk_pool, d.chunk_pool, s), "upload"); CK(put(e->b_pool_chunk0, t.pool_chunk0, d.pool_chunk0, s), "upload");
+    CK(put(e->b_merge_list, t.merge_list, d.merge_list, s), "upload");
     d.n_chunks = t.n_chunks; d.n_merge = t.n_merge; d.merge_smem = t.merge_smem;
-    CK(up(e->b_lbm_off, t.lbm_off, s), "upload");
-    d.lbm_off = (const uint32_t*)e->b_lbm_off.p;
+    CK(put(e->b_lbm_off, t.lbm_off, d.lbm_off, s), "upload");
     d.place_bits = t.place_bits;
     d.n_pos = t.n_pos; d.n_pools = t.n_pools;
-    d.pool_off = (const uint32_t*)e->b_pool_off.p; d.pos_pool = (const uint32_t*)e->b_pos_pool.p;
-    d.pos_slot = (const uint32_t*)e->b_pos_slot.p; d.pos_rank = (const uint32_t*)e->b_pos_rank.p;
-    d.slot_pos = (const uint32_t*)e->b_slot_pos.p; d.rank_slot = (const uint32_t*)e->b_rank_slot.p;
-    d.pos_label_lo = (const uint64_t*)e->b_pos_label_lo.p; d.pos_label_hi = (const uint64_t*)e->b_pos_label_hi.p;
-    CK(up(e->b_pos_label_x, t.pos_label_x, s), "upload");
-    d.pos_label_x = (const uint64_t*)e->b_pos_label_x.p;
+    CK(put(e->b_pos_label_x, t.pos_label_x, d.pos_label_x, s), "upload");
     e->v_workers = t.v_workers;
     e->pools_dirty = true;
-    e->host_loads = true;
   }
   if (t.v_loads != e->v_loads) {   // heartbeat deltas applied on the host (cordum_workers_update)
     e->v_loads = t.v_loads;
     e->pools_dirty = true;
-    e->host_loads = true;
   }
   d.wide = t.wide;
   d.wide_words = WIDE_WORDS(t.wide);
@@ -346,7 +332,6 @@ int sync_dicts(cordum_engine* e) {
   return CORDUM_OK;
 }
 
-// The kernels' view of the tables with the derived pointers of one set.
 // Parameters of the peer push for table parity p; returns this rank's full table of that parity (inside its IPC buffer).
 uint8_t* peer_push_params(const cordum_engine* e, int p, PeerPush& G) {
   const auto& P = e->peers;
@@ -376,6 +361,7 @@ int leave_tick_mode(cordum_engine* e) {
   return CORDUM_OK;
 }
 
+// The kernels' view of the tables with the derived pointers of one set.
 DeviceTables view(const cordum_engine* e, int set) {
   DeviceTables d = e->dt;
   const auto& D = e->ds[set];
@@ -393,16 +379,104 @@ DeviceTables view(const cordum_engine* e, int set) {
   return d;
 }
 
+// Kernels one refresh of the derived worker tables launches (worker_chunk, worker_merge).
+uint32_t refresh_launches(const cordum_engine* e) { return (e->dt.n_chunks ? 1 : 0) + (e->dt.n_merge ? 1 : 0); }
+
+// The set the next heartbeat epoch is refreshed into: the one after the latest, once the route kernels that still read it
+// (launched kSets-1 epochs ago) have finished.  Returns the set, or an error code (< 0).
+int claim_set(cordum_engine* e) {
+  const int target = (e->cur + 1) % kSets;
+  for (cordum_batch* b : e->batches)
+    if (b->launched && b->table_set == target) { CK(cudaStreamWaitEvent(e->s_tables, b->ev2, 0), "wait route"); b->launched = false; }
+  return target;
+}
+
+// The refresh of set `target` has been enqueued on the tables stream (`launches` kernels): dispatches route on it from here on.
+int publish_set(cordum_engine* e, int target, uint32_t launches) {
+  CK(cudaEventRecord(e->ds[target].ready, e->s_tables), "event record");
+  e->launches += launches;
+  e->cur = target;
+  e->pools_dirty = false;
+  return CORDUM_OK;
+}
+
+// Refresh kernels of a heartbeat epoch on the tables stream, into set `target`.  loads: the full slot-ordered load table
+// they read (null: the set's own copy); loads_read (optional) is recorded once they have consumed it.
+int refresh_on_tables_stream(cordum_engine* e, int target, const Load16* loads, cudaEvent_t loads_read) {
+  DeviceTables tv = view(e, target);
+  if (loads) tv.loads = loads;
+  CK(launch_worker_pools(tv, e->s_tables, loads_read), "worker-table refresh kernels");
+  return publish_set(e, target, refresh_launches(e));
+}
+
+// One heartbeat epoch as captured into a graph on stream s: the staged slice of parity p to the device - into this rank's
+// slice of the peer table of that parity, then pushed to every peer, when the peers exchange it - then the refresh
+// kernels of `set` on the full table.
+cudaError_t enqueue_heartbeat(cordum_engine* e, cudaStream_t s, int p, int set, bool peers) {
+  uint8_t* table = (uint8_t*)e->gather[p].p;
+  DeviceTables tv = view(e, set);
+  cudaError_t ce = cudaSuccess;
+  if (peers) {
+    // the staging buffer carries the epoch number behind the slice; the push kernel - whose parameters the graph bakes
+    // in - reads the epoch it announces and waits for from device memory
+    const size_t slice_bytes = (size_t)e->peers.per * sizeof(Load16);
+    PeerPush G{};
+    table = peer_push_params(e, p, G);
+    ce = cudaMemcpyAsync((void*)G.my_slice, e->stage[p], slice_bytes, cudaMemcpyHostToDevice, s);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync((void*)G.epoch_ptr, (const uint8_t*)e->stage[p] + slice_bytes, 4, cudaMemcpyHostToDevice, s);
+    if (ce == cudaSuccess) ce = launch_peer_push(G, s);
+  } else {
+    ce = cudaMemcpyAsync(table, e->stage[p], (size_t)e->host->tables().n_slots * sizeof(Load16), cudaMemcpyHostToDevice, s);
+  }
+  tv.loads = (const Load16*)table;
+  return ce != cudaSuccess ? ce : launch_worker_pools(tv, s, nullptr);
+}
+
+// The pinned heartbeat staging, large enough for a slice of `bytes`.  Both graph caches bake its pointers in.
+int grow_staging(cordum_engine* e, size_t bytes) {
+  if (e->stage[0] && e->stage_cap >= bytes) return CORDUM_OK;
+  CK(cudaDeviceSynchronize(), "sync before staging growth");
+  for (auto& p : e->stage) { if (p) cudaFreeHost(p); p = nullptr; }
+  for (auto& p : e->stage) CK(cudaHostAlloc((void**)&p, bytes + 64, cudaHostAllocDefault), "pinned heartbeat staging");
+  e->stage_cap = bytes;
+  for (auto& kv : e->ing_graphs) cudaGraphExecDestroy(kv.second);
+  e->ing_graphs.clear();
+  for (auto& kv : e->tick.graphs) cudaGraphExecDestroy(kv.second);
+  e->tick.graphs.clear();
+  return CORDUM_OK;
+}
+
+// The gathered load tables of both parities, large enough for `bytes`: nothing may still read the old buffers, and the
+// captured graphs that bake their pointers in are stale.
+int grow_gather(cordum_engine* e, size_t bytes) {
+  if (e->gather[0].cap >= bytes && e->gather[1].cap >= bytes) return CORDUM_OK;
+  CK(cudaDeviceSynchronize(), "sync before gather buffer allocation");
+  for (auto& b : e->gather) CK(b.reserve(bytes), "alloc gather buffer");
+  e->tables_gen++;
+  return CORDUM_OK;
+}
+
+// What policy_kernel and route_kernel of batch b read and write, on tables t.  policy_and_route (CORDUM_MODE_POLICY_AND_ROUTE):
+// approvals are honoured, and policy_kernel compacts the dispatchable jobs into the batch's route list for route_kernel.
+KParams batch_params(const cordum_batch* b, const DeviceTables& t, bool policy_and_route) {
+  KParams P{};
+  P.t = t;
+  device_records(b, P.recs);
+  P.out = b->d_out;
+  P.n_jobs = b->n;
+  P.honor_approved = policy_and_route ? 1u : 0u;
+  if (policy_and_route) { P.route_count = reinterpret_cast<uint32_t*>(b->d_route); P.route_list = b->d_route + 2; }
+  return P;
+}
+
 // worker-table refresh kernels for a new heartbeat epoch, into the set that is NOT being read.  dev_loads: the full slot-ordered
 // load table already in HBM (produced on `producer`), or null to take the host tables' loads.  Called with both mutexes held.
 int refresh_pools(cordum_engine* e, const void* dev_loads, cudaStream_t producer) {
   cordum::NvtxRange nvtx_("cordum:worker_refresh");
   if (!e->pools_dirty && !dev_loads) return CORDUM_OK;
-  const int target = (e->cur + 1) % kSets;
+  const int target = claim_set(e);
+  if (target < 0) return target;
   auto& D = e->ds[target];
-  // route kernels that still read the target set (launched kSets-1 epochs ago) must have finished
-  for (cordum_batch* b : e->batches)
-    if (b->launched && b->table_set == target) { CK(cudaStreamWaitEvent(e->s_tables, b->ev2, 0), "wait route"); b->launched = false; }
   const HostTables& t = e->host->tables();
   const size_t bytes = (size_t)t.n_slots * sizeof(Load16);
   if (dev_loads) {
@@ -417,16 +491,10 @@ int refresh_pools(cordum_engine* e, const void* dev_loads, cudaStream_t producer
     CK(cudaEventRecord(e->ev_copy, e->s_copy), "event record");
     CK(cudaStreamWaitEvent(producer, e->ev_copy, 0), "order producer after copy");
     CK(cudaStreamWaitEvent(e->s_tables, e->ev_copy, 0), "order refresh after copy");
-    e->host_loads = false;
   } else if (bytes) {
     CK(cudaMemcpyAsync(D.loads.p, t.loads.data(), bytes, cudaMemcpyHostToDevice, e->s_tables), "H2D loads");
   }
-  CK(launch_worker_pools(view(e, target), e->s_tables, D.loads_read), "worker-table refresh kernels");
-  e->launches += (e->dt.n_chunks ? 1 : 0) + (e->dt.n_merge ? 1 : 0);
-  CK(cudaEventRecord(D.ready, e->s_tables), "event record");
-  e->cur = target;
-  e->pools_dirty = false;
-  return CORDUM_OK;
+  return refresh_on_tables_stream(e, target, nullptr, D.loads_read);
 }
 
 int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool copy_out) {
@@ -445,7 +513,7 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
   b->last_copy_out = copy_out;
   if (b->pending) { CK(cudaStreamSynchronize(b->stream), "wait previous"); b->pending = false; b->enc_inflight = false; }
   CK(cudaSetDevice(e->device), "cudaSetDevice");
-  KParams P;
+  DeviceTables tv;
   cudaEvent_t ev_ready = nullptr;
   if (int rc = leave_tick_mode(e)) return rc;
   // e->mu is held until every launch of this dispatch is enqueued: a table sync on another thread (first sight of a
@@ -460,7 +528,7 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
     if (rc) return rc;
     rc = refresh_pools(e, nullptr, nullptr);
     if (rc) return rc;
-    P.t = view(e, e->cur);
+    tv = view(e, e->cur);
     b->table_set = e->cur;
     ev_ready = e->ds[e->cur].ready;
   }
@@ -478,15 +546,8 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
     b->resident = true;
   }
   if (timed) CK(cudaEventRecord(b->ev1, s), "event");
-  device_records(b, P.recs);
-  P.out = b->d_out;
-  P.n_jobs = b->n;
-  P.honor_approved = mode == CORDUM_MODE_POLICY_AND_ROUTE ? 1u : 0u;
-  P.route_count = nullptr; P.route_list = nullptr;
-  if (mode == CORDUM_MODE_POLICY_AND_ROUTE) {   // policy_kernel compacts the dispatchable jobs for route_kernel
-    P.route_count = reinterpret_cast<uint32_t*>(b->d_route); P.route_list = b->d_route + 2;
-    CK(cudaMemsetAsync(b->d_route, 0, sizeof(uint32_t), s), "reset route count");
-  }
+  const KParams P = batch_params(b, tv, mode == CORDUM_MODE_POLICY_AND_ROUTE);
+  if (P.route_count) CK(cudaMemsetAsync(b->d_route, 0, sizeof(uint32_t), s), "reset route count");
   // policy_kernel needs no worker state: it is NOT ordered after the heartbeat exchange / worker-table refresh kernels
   if (mode != CORDUM_MODE_ROUTE_ONLY) {
     CK(launch_policy(P, e->sm_count, s), "policy_kernel");
@@ -570,7 +631,6 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
   std::free(b->slot_of);
-  b->d_env.release(); b->d_work.release();
   if (b->h_fallback) cudaFreeHost(b->h_fallback);
   for (cudaEvent_t ev : {b->ev0, b->ev1, b->evm, b->ev2, b->ev3}) if (ev) cudaEventDestroy(ev);
   if (b->stream) cudaStreamDestroy(b->stream);
@@ -633,26 +693,13 @@ int ingest(cordum_engine* e, const cordum_worker_load* slice, uint32_t first_slo
   const bool use_peers = e->peers.ready && e->peers.world > 1 && e->peers.world == e->xworld && e->peers.per == per;
   if (e->xworld == 1 || use_peers) {
     // One graph launch: H2D of the slice -> [gather of all ranks' slices over peer memory] -> worker_chunk -> worker_merge.
-    if (e->gather[g].cap < bytes) {
-      CK(cudaDeviceSynchronize(), "sync before gather buffer allocation");
-      CK(e->gather[g].reserve(bytes), "alloc gather buffer");
-      e->tables_gen++;
-    }
-    if (e->ing_cap < slice_bytes) {
-      CK(cudaDeviceSynchronize(), "sync before staging growth");
-      for (auto& p : e->ing_stage) { if (p) cudaFreeHost(p); p = nullptr; }
-      for (auto& p : e->ing_stage) CK(cudaHostAlloc((void**)&p, slice_bytes + 64, cudaHostAllocDefault), "pinned heartbeat staging");
-      e->ing_cap = slice_bytes;
-      for (auto& kv : e->ing_graphs) cudaGraphExecDestroy(kv.second);
-      e->ing_graphs.clear();
-    }
+    if (int rc = grow_gather(e, bytes)) return rc;
+    if (int rc = grow_staging(e, slice_bytes)) return rc;
     CK(cudaEventSynchronize(e->gather_free[g]), "wait staging");   // the epoch two back has consumed this staging / table buffer
-    std::memcpy(e->ing_stage[g], slice, slice_bytes);
-    *reinterpret_cast<uint32_t*>((uint8_t*)e->ing_stage[g] + slice_bytes) = (uint32_t)e->xepoch;   // the epoch, behind the slice
-    const int target = (e->cur + 1) % kSets;
-    auto& D = e->ds[target];
-    for (cordum_batch* b : e->batches)   // route kernels that still read the target set
-      if (b->launched && b->table_set == target) { CK(cudaStreamWaitEvent(e->s_tables, b->ev2, 0), "wait route"); b->launched = false; }
+    std::memcpy(e->stage[g], slice, slice_bytes);
+    *reinterpret_cast<uint32_t*>((uint8_t*)e->stage[g] + slice_bytes) = (uint32_t)e->xepoch;   // the epoch, behind the slice
+    const int target = claim_set(e);
+    if (target < 0) return target;
     const auto key = std::make_tuple(target, g, e->tables_gen);
     cudaGraphExec_t ge = nullptr;
     auto it = e->ing_graphs.find(key);
@@ -662,19 +709,7 @@ int ingest(cordum_engine* e, const cordum_worker_load* slice, uint32_t first_slo
       CK(launch_configure(), "kernel attributes");
       cudaStream_t S = e->s_tables;
       CK(cudaStreamBeginCapture(S, cudaStreamCaptureModeThreadLocal), "begin capture");
-      cudaError_t ce = cudaSuccess;
-      uint8_t* table = (uint8_t*)e->gather[g].p;
-      DeviceTables tv = view(e, target);
-      tv.loads = (const Load16*)table;
-      if (use_peers) {
-        PeerPush G{};
-        table = peer_push_params(e, g, G);
-        tv.loads = (const Load16*)table;
-        ce = cudaMemcpyAsync((void*)G.my_slice, e->ing_stage[g], slice_bytes, cudaMemcpyHostToDevice, S);
-        if (ce == cudaSuccess) ce = cudaMemcpyAsync((void*)G.epoch_ptr, (const uint8_t*)e->ing_stage[g] + slice_bytes, 4, cudaMemcpyHostToDevice, S);
-        if (ce == cudaSuccess) ce = launch_peer_push(G, S);
-      } else ce = cudaMemcpyAsync(table, e->ing_stage[g], slice_bytes, cudaMemcpyHostToDevice, S);
-      if (ce == cudaSuccess) ce = launch_worker_pools(tv, S, nullptr);
+      const cudaError_t ce = enqueue_heartbeat(e, S, g, target, use_peers);
       cudaGraph_t gr = nullptr;
       cudaError_t ee = cudaStreamEndCapture(S, &gr);
       if (ce != cudaSuccess || ee != cudaSuccess) { if (gr) cudaGraphDestroy(gr); return fail(e, ce != cudaSuccess ? ce : ee, "capture of the ingest graph"); }
@@ -685,17 +720,9 @@ int ingest(cordum_engine* e, const cordum_worker_load* slice, uint32_t first_slo
     }
     CK(cudaGraphLaunch(ge, e->s_tables), "graph launch");
     CK(cudaEventRecord(e->gather_free[g], e->s_tables), "event record");
-    CK(cudaEventRecord(D.ready, e->s_tables), "event record");
-    e->launches += (e->dt.n_chunks ? 1 : 0) + (e->dt.n_merge ? 1 : 0) + (use_peers ? 1 : 0);
-    e->cur = target;
-    e->pools_dirty = false;
-    e->host_loads = false;
-    return CORDUM_OK;
+    return publish_set(e, target, refresh_launches(e) + (use_peers ? 1 : 0));
   }
-  if (e->gather[g].cap < bytes) {   // first use / registry grew: nothing may still read the old buffer
-    CK(cudaDeviceSynchronize(), "sync before gather buffer allocation");
-    CK(e->gather[g].reserve(bytes), "alloc gather buffer");
-  }
+  if (int rc = grow_gather(e, bytes)) return rc;
   uint8_t* table = (uint8_t*)e->gather[g].p;
   // the refresh two epochs ago read this buffer
   CK(cudaStreamWaitEvent(e->s_xchg, e->gather_free[g], 0), "wait gather buffer");
@@ -705,20 +732,11 @@ int ingest(cordum_engine* e, const cordum_worker_load* slice, uint32_t first_slo
     if (rc) return nccl_fail(e, rc, "ncclAllGather");
   }
   CK(cudaEventRecord(e->ev_xchg, e->s_xchg), "event record");
-  const int target = (e->cur + 1) % kSets;
-  auto& D = e->ds[target];
-  for (cordum_batch* b : e->batches)   // route kernels that still read the target set
-    if (b->launched && b->table_set == target) { CK(cudaStreamWaitEvent(e->s_tables, b->ev2, 0), "wait route"); b->launched = false; }
+  const int target = claim_set(e);
+  if (target < 0) return target;
   CK(cudaStreamWaitEvent(e->s_tables, e->ev_xchg, 0), "order refresh after exchange");
-  DeviceTables tv = view(e, target);
-  tv.loads = (const Load16*)table;   // the refresh reads the gathered table in place
-  CK(launch_worker_pools(tv, e->s_tables, e->gather_free[g]), "worker-table refresh kernels");
-  e->launches += (e->dt.n_chunks ? 1 : 0) + (e->dt.n_merge ? 1 : 0);
-  CK(cudaEventRecord(D.ready, e->s_tables), "event record");
-  e->cur = target;
-  e->pools_dirty = false;
-  e->host_loads = false;
-  return CORDUM_OK;
+  // the refresh reads the gathered table in place
+  return refresh_on_tables_stream(e, target, (const Load16*)table, e->gather_free[g]);
 }
 }  // namespace
 
@@ -758,24 +776,7 @@ int tick_graph(cordum_engine* e, cordum_batch* bn, cordum_batch* bp, int phase, 
   // ---- A: heartbeat epoch, behind the heartbeat branch of the previous tick (a graph of its own, on the other stream)
   CKC(cudaStreamWaitEvent(T.sa, T.ev_fork, 0), "fork");
   CKC(cudaStreamWaitEvent(T.sa, T.refreshed[parity ^ 1], cudaEventWaitExternal), "order heartbeat epochs");
-  if (W) {
-    uint8_t* table = (uint8_t*)e->gather[parity].p;
-    DeviceTables tv = view(e, set_new);
-    tv.loads = (const Load16*)table;
-    if (e->peers.ready && e->peers.world > 1) {
-      // the staging buffer carries the epoch number behind the slice; the push kernel - whose parameters the graph bakes
-      // in - reads the epoch it announces and waits for from device memory
-      PeerPush G{};
-      table = peer_push_params(e, parity, G);
-      tv.loads = (const Load16*)table;
-      CKC(cudaMemcpyAsync((void*)G.my_slice, T.h_slice[parity], (size_t)e->peers.per * sizeof(Load16), cudaMemcpyHostToDevice, T.sa), "H2D heartbeat slice");
-      CKC(cudaMemcpyAsync((void*)G.epoch_ptr, (const uint8_t*)T.h_slice[parity] + (size_t)e->peers.per * sizeof(Load16), 4, cudaMemcpyHostToDevice, T.sa), "H2D epoch");
-      CKC(launch_peer_push(G, T.sa), "peer push");
-    } else {
-      CKC(cudaMemcpyAsync(table, T.h_slice[parity], (size_t)W * sizeof(Load16), cudaMemcpyHostToDevice, T.sa), "H2D heartbeats");
-    }
-    CKC(launch_worker_pools(tv, T.sa, nullptr), "worker-table refresh kernels");
-  }
+  if (W) CKC(enqueue_heartbeat(e, T.sa, parity, set_new, e->peers.ready && e->peers.world > 1), "heartbeat epoch");
   CKC(cudaEventRecordWithFlags(T.refreshed[parity], T.sa, cudaEventRecordExternal), "publish heartbeat epoch");
   CKC(cudaEventRecord(T.ev_a, T.sa), "join");
   // ---- C: route of the previous batch on the previous epoch's tables, once the previous tick (policy of that batch, refresh
@@ -783,21 +784,12 @@ int tick_graph(cordum_engine* e, cordum_batch* bn, cordum_batch* bp, int phase, 
   if (bp && bp->n) {
     CKC(cudaStreamWaitEvent(T.sc, T.ev_fork, 0), "fork");
     CKC(cudaStreamWaitEvent(T.sc, T.done[parity ^ 1], cudaEventWaitExternal), "wait previous tick");
-    KParams P{};
-    P.t = view(e, set_old);
-    device_records(bp, P.recs);
-    P.out = bp->d_out; P.n_jobs = bp->n; P.honor_approved = 1u;
-    P.route_count = reinterpret_cast<uint32_t*>(bp->d_route); P.route_list = bp->d_route + 2;
-    CKC(launch_route(P, false, e->sm_count, T.sc, tick_share()), "route_kernel");
+    CKC(launch_route(batch_params(bp, view(e, set_old), true), false, e->sm_count, T.sc, tick_share()), "route_kernel");
     CKC(cudaEventRecord(T.ev_c, T.sc), "join");
   }
   // ---- B: policy of the new batch
   if (bn && bn->n) {
-    KParams P{};
-    P.t = view(e, set_old);   // policy_kernel reads no worker state
-    device_records(bn, P.recs);
-    P.out = bn->d_out; P.n_jobs = bn->n; P.honor_approved = 1u;
-    P.route_count = reinterpret_cast<uint32_t*>(bn->d_route); P.route_list = bn->d_route + 2;
+    const KParams P = batch_params(bn, view(e, set_old), true);   // policy_kernel reads no worker state
     // this batch's previous use was routed by the tick before this one (only two batches alternate): that route still
     // reads what this policy run overwrites
     if (bn_routed_last_tick) CKC(cudaStreamWaitEvent(S, T.done[parity ^ 1], cudaEventWaitExternal), "wait previous route of this batch");
@@ -851,12 +843,7 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
       const int pp = (int)((T.n + 5) % 6);   // phase of the previous tick
       cudaStream_t S = T.s[parity];
       CK(cudaStreamWaitEvent(S, T.done[pp & 1], 0), "wait previous tick");
-      KParams P{};
-      P.t = view(e, pp % 3);
-      device_records(bp, P.recs);
-      P.out = bp->d_out; P.n_jobs = bp->n; P.honor_approved = 1u;
-      P.route_count = reinterpret_cast<uint32_t*>(bp->d_route); P.route_list = bp->d_route + 2;
-      CK(launch_route(P, false, e->sm_count, S), "route_kernel");
+      CK(launch_route(batch_params(bp, view(e, pp % 3), true), false, e->sm_count, S), "route_kernel");
       if (bp->n) e->launches++;
       T.prev = nullptr;
     }
@@ -872,22 +859,10 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
   CK(cudaEventSynchronize(T.done[parity]), "wait staging");
   const auto t1 = now();
   const size_t bytes = (size_t)n_slice * sizeof(Load16);
-  if (T.h_cap < bytes) {
-    for (cudaStream_t st : T.s) CK(cudaStreamSynchronize(st), "drain before staging growth");
-    for (auto& p : T.h_slice) { if (p) cudaFreeHost(p); p = nullptr; }
-    for (auto& p : T.h_slice) CK(cudaHostAlloc((void**)&p, bytes + 64, cudaHostAllocDefault), "pinned heartbeat staging");
-    T.h_cap = bytes;
-    for (auto& kv : T.graphs) cudaGraphExecDestroy(kv.second);   // they bake the staging pointers in
-    T.graphs.clear();
-  }
-  if (bytes) std::memcpy(T.h_slice[parity], slice, bytes);
-  *reinterpret_cast<uint32_t*>((uint8_t*)T.h_slice[parity] + bytes) = (uint32_t)(++e->xepoch);   // the epoch (shared with cordum_workers_ingest), behind the slice
-  if (e->gather[parity].cap < (size_t)W * sizeof(Load16)) {
-    CK(cudaDeviceSynchronize(), "sync before gather buffer allocation");
-    CK(e->gather[parity].reserve((size_t)W * sizeof(Load16)), "alloc gather buffer");
-    CK(e->gather[parity ^ 1].reserve((size_t)W * sizeof(Load16)), "alloc gather buffer");
-    e->tables_gen++;
-  }
+  if (int rc = grow_staging(e, bytes)) return rc;
+  if (bytes) std::memcpy(e->stage[parity], slice, bytes);
+  *reinterpret_cast<uint32_t*>((uint8_t*)e->stage[parity] + bytes) = (uint32_t)(++e->xepoch);   // the epoch (shared with cordum_workers_ingest), behind the slice
+  if (int rc = grow_gather(e, (size_t)W * sizeof(Load16))) return rc;
   const auto t2 = now();
   cudaGraphExec_t ge = nullptr;
   // Ticks up to n-2 have finished when tick n starts (stream order + the route branch's wait); tick n-1 may still run.
@@ -908,9 +883,9 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
       acc[0] = acc[1] = acc[2] = acc[3] = 0;
     }
   }
-  e->launches += (W ? (e->dt.n_chunks ? 1 : 0) + (e->dt.n_merge ? 1 : 0) + (e->peers.ready && e->peers.world > 1 ? 1 : 0) : 0) + (bn->n ? 1 : 0) + (T.prev && T.prev->n ? 1 : 0);
+  e->launches += (W ? refresh_launches(e) + (e->peers.ready && e->peers.world > 1 ? 1 : 0) : 0) + (bn->n ? 1 : 0) + (T.prev && T.prev->n ? 1 : 0);
   e->cur = phase % 3;   // the set this tick refreshed (a later plain dispatch continues from it)
-  e->pools_dirty = false; e->host_loads = false;
+  e->pools_dirty = false;
   bn->tick_no = T.n;
   T.prev = bn;
   T.n++;
@@ -1035,25 +1010,15 @@ void cordum_engine_destroy(cordum_engine* e) {
     for (cordum_batch* b : live) batch_release(b);
   }
   for (auto& kv : e->ing_graphs) cudaGraphExecDestroy(kv.second);
-  for (auto& p : e->ing_stage) if (p) cudaFreeHost(p);
+  for (auto& p : e->stage) if (p) cudaFreeHost(p);
   for (auto& kv : e->tick.graphs) cudaGraphExecDestroy(kv.second);
   for (cudaStream_t st : {e->tick.s[0], e->tick.s[1], e->tick.sa, e->tick.sc}) if (st) cudaStreamDestroy(st);
   for (cudaEvent_t ev : {e->tick.ev_fork, e->tick.ev_a, e->tick.ev_c, e->tick.ev_join, e->tick.done[0], e->tick.done[1], e->tick.refreshed[0], e->tick.refreshed[1]}) if (ev) cudaEventDestroy(ev);
-  for (auto& p : e->tick.h_slice) if (p) cudaFreeHost(p);
   for (int q = 0; q < e->peers.world && e->peers.ready; ++q) if (q != e->peers.rank && e->peers.base[q]) cudaIpcCloseMemHandle(e->peers.base[q]);
   if (e->peers.mine) cudaFree(e->peers.mine);
   for (cordum_envelopes* env : e->env_sets) cudaFreeHost(env);
   e->env_sets.clear();
-  DevBuf* all[] = {&e->b_dicts, &e->b_rows, &e->b_row_check,
-                   &e->b_req_need, &e->b_lab_need, &e->b_rule_dec, &e->b_tenant_mcp, &e->b_eff_mcp, &e->b_eff_topic, &e->b_pos2rule,
-                   &e->b_sum_tenant, &e->b_sum_topic, &e->b_sum_cap, &e->b_sum_pack, &e->b_sum_actor, &e->b_sum_combo, &e->b_sum_risk,
-                   &e->b_topic_pool_off, &e->b_topic_pool_cnt, &e->b_pool_list, &e->b_pool_req_mask, &e->b_pool_req_nonempty,
-                   &e->b_pool_off, &e->b_pos_pool, &e->b_pos_slot, &e->b_pos_rank, &e->b_slot_pos, &e->b_rank_slot,
-                   &e->b_pos_label_lo, &e->b_pos_label_hi, &e->b_rule_need_x, &e->b_pool_req_x, &e->b_req_blank_x, &e->b_pos_label_x, &e->b_flush, &e->b_lbm_off, &e->b_rank_pos,
-                   &e->b_chunk_pool, &e->b_pool_chunk0, &e->b_merge_list};
-  for (DevBuf* b : all) b->release();
   for (auto& D : e->ds) {
-    for (DevBuf* b : {&D.loads, &D.pos_key, &D.ckey, &D.skey, &D.pool_sorted, &D.pool_nok, &D.pool_done, &D.lbm, &D.lbest, &D.pool_best, &D.pool_mincnt}) b->release();
     if (D.ready) cudaEventDestroy(D.ready);
     if (D.loads_read) cudaEventDestroy(D.loads_read);
   }
@@ -1062,7 +1027,6 @@ void cordum_engine_destroy(cordum_engine* e) {
   if (e->s_tables) cudaStreamDestroy(e->s_tables);
   if (e->s_copy) cudaStreamDestroy(e->s_copy);
   if (e->nccl_comm && nccl_api()) nccl_api()->CommDestroy(e->nccl_comm);
-  for (auto& b : e->gather) b.release();
   for (auto& ev : e->gather_free) if (ev) cudaEventDestroy(ev);
   if (e->ev_xchg) cudaEventDestroy(e->ev_xchg);
   if (e->s_xchg) cudaStreamDestroy(e->s_xchg);
