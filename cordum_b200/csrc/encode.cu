@@ -15,7 +15,8 @@
 //
 // What stays on the host: anything that needs Unicode tables (TrimSpace / EqualFold / ToLower on non-ASCII text), the
 // first sight of a topic or of an effective config (the host has to compute pass-rows / parse JSON), and strings longer
-// than kMaxStr.  A job that meets one of these raises the batch's fallback flag and the host encodes the batch instead.
+// than kMaxStr, and a selective placement pair (tables.h DeviceTables.sel_*).  A job that meets one of these raises the
+// batch's fallback flag and the host encodes the batch instead.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -316,6 +317,7 @@ __global__ void __launch_bounds__(128) encode_job_kernel(EncodeParams P) {
       if (val.n) {
         bit = dict_find<false>(E, DD_PLACE_PAIR, Str{scratch, 4 + key.n + val.n}, hash_pair(key, val, scratch), kMiss);
         if (bit == kMiss) flags |= JF_PLACE_UNSAT;
+        else if (bit & CORDUM_SEL_TAG) bad = true;   // a selective pair: the host encoder writes the batch's selective list
       } else {
         bit = find_exact(E, DD_PLACE_KEY, key, kMiss);
         if (bit == kMiss) bit = E.place_any_bit;   // no worker carries this key: any labelled worker passes

@@ -91,6 +91,7 @@ struct cordum_engine {
   DevBuf b_rule_need_x, b_pool_req_x, b_req_blank_x, b_pos_label_x;   // wide masks (tables.h WideLayout)
   DevBuf b_pool_off, b_pos_pool, b_pos_slot, b_pos_rank, b_slot_pos, b_rank_slot, b_pos_label_lo, b_pos_label_hi;
   DevBuf b_flush, b_lbm_off, b_rank_pos, b_chunk_pool, b_pool_chunk0, b_merge_list;
+  DevBuf b_sel_off, b_sel_pos, b_pos_sel_off, b_pos_sel;   // selective placement pairs (tables.h DeviceTables.sel_*)
   DevBuf b_dicts;                // device encoder: dictionary images + side arrays (Host::export_dicts)
   EncodeTables et{};             // rebased onto b_dicts
   uint64_t v_dict = ~0ull;
@@ -116,7 +117,7 @@ struct cordum_engine {
     cordum_batch* prev = nullptr;                          // its policy ran in the previous tick; its route is due
     uint64_t n = 0;                                        // ticks so far
     bool active = false;                                   // ticks have been issued since the last plain dispatch / ingest
-    std::map<std::tuple<cordum_batch*, cordum_batch*, int, uint32_t, uint32_t, uint64_t>, cudaGraphExec_t> graphs;
+    std::map<std::tuple<cordum_batch*, cordum_batch*, int, uint32_t, uint32_t, uint32_t, uint64_t>, cudaGraphExec_t> graphs;
   } tick;
   // ---- peer-memory heartbeat exchange (cordum_peer_export / cordum_peer_import)
   struct Peers {
@@ -157,6 +158,9 @@ struct cordum_batch {
   uint64_t *h_wide = nullptr, *d_wide = nullptr;   // wide-mask rows (tables.h WideLayout), allocated on first need
   uint64_t wide_cap = 0;         // 64-bit words allocated at each of the two
   uint32_t wide_words = 0;       // row width of the encoded batch
+  uint32_t *h_sel = nullptr, *d_sel = nullptr;   // the selective list (tables.h JobRecords), allocated on first need
+  size_t sel_cap = 0;            // 32-bit words allocated at each of the two
+  uint32_t n_sel_jobs = 0, sel_words = 0;   // of the encoded batch: listed jobs, words in use
   uint32_t* slot_of = nullptr;   // host: position of caller job j in the sorted records
   // device-side encode (cordum_encode_device)
   bool device_encoded = false, host_records_valid = true;
@@ -196,6 +200,9 @@ void device_records(const cordum_batch* b, JobRecords& r) {
   r.job = (const JobRec*)b->d_cols;
   r.route = (const RouteRec*)(b->d_cols + (size_t)b->n * sizeof(JobRec));
   r.wide = b->wide_words ? b->d_wide : nullptr;
+  r.n_sel_jobs = b->n_sel_jobs;
+  r.sel_jobs = b->n_sel_jobs ? reinterpret_cast<const uint2*>(b->d_sel) : nullptr;
+  r.sel_extra = b->n_sel_jobs ? b->d_sel + 2 * (size_t)b->n_sel_jobs : nullptr;
 }
 
 // Uploads a host table into b and points the kernels' view (field) at it.
@@ -298,6 +305,9 @@ int sync_tables(cordum_engine* e) {
     d.place_bits = t.place_bits;
     d.n_pos = t.n_pos; d.n_pools = t.n_pools;
     CK(put(e->b_pos_label_x, t.pos_label_x, d.pos_label_x, s), "upload");
+    CK(put(e->b_sel_off, t.sel_off, d.sel_off, s), "upload"); CK(put(e->b_sel_pos, t.sel_pos, d.sel_pos, s), "upload");
+    CK(put(e->b_pos_sel_off, t.pos_sel_off, d.pos_sel_off, s), "upload"); CK(put(e->b_pos_sel, t.pos_sel, d.pos_sel, s), "upload");
+    d.n_sel = t.n_sel;
     e->v_workers = t.v_workers;
     e->pools_dirty = true;
   }
@@ -543,6 +553,7 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
     CK(cudaEventRecord(b->ev0, s), "event");
     CK(cudaMemcpyAsync(b->d_cols, b->h_cols, slab_bytes(b->n), cudaMemcpyHostToDevice, s), "H2D columns");
     if (b->wide_words) CK(cudaMemcpyAsync(b->d_wide, b->h_wide, (size_t)b->n * b->wide_words * 8, cudaMemcpyHostToDevice, s), "H2D wide masks");
+    if (b->sel_words) CK(cudaMemcpyAsync(b->d_sel, b->h_sel, (size_t)b->sel_words * 4, cudaMemcpyHostToDevice, s), "H2D selective list");
     b->resident = true;
   }
   if (timed) CK(cudaEventRecord(b->ev1, s), "event");
@@ -557,7 +568,7 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
   if (mode != CORDUM_MODE_POLICY_ONLY) {
     CK(cudaStreamWaitEvent(s, ev_ready, 0), "wait worker tables");
     CK(launch_route(P, mode == CORDUM_MODE_ROUTE_ONLY, e->sm_count, s), "route_kernel");
-    if (b->n) e->launches++;
+    e->launches += route_launches(P);
   }
   CK(cudaEventRecord(b->ev2, s), "event");
   b->launched = true;
@@ -627,6 +638,8 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->d_cols) cudaFree(b->d_cols);
   if (b->h_wide) cudaFreeHost(b->h_wide);
   if (b->d_wide) cudaFree(b->d_wide);
+  if (b->h_sel) cudaFreeHost(b->h_sel);
+  if (b->d_sel) cudaFree(b->d_sel);
   if (b->h_out) cudaFreeHost(b->h_out);
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
@@ -754,7 +767,8 @@ int tick_graph(cordum_engine* e, cordum_batch* bn, cordum_batch* bp, int phase, 
   // phase = tick number mod 6: stream / staging / gather-buffer parity = phase & 1, derived-table set = phase % 3
   auto& T = e->tick;
   const uint32_t W = e->host->tables().n_slots;
-  const auto key = std::make_tuple(bn, bp, phase + (bn_routed_last_tick ? 8 : 0), bn ? bn->n : 0u, bp ? bp->n : 0u, e->tables_gen);
+  const auto key = std::make_tuple(bn, bp, phase + (bn_routed_last_tick ? 8 : 0), bn ? bn->n : 0u, bp ? bp->n : 0u,
+                                   bp ? bp->n_sel_jobs : 0u, e->tables_gen);
   auto it = T.graphs.find(key);
   if (it != T.graphs.end()) { *out = it->second; return CORDUM_OK; }
   if (T.graphs.size() > 96) {   // stale generations / batches: start over
@@ -843,8 +857,9 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
       const int pp = (int)((T.n + 5) % 6);   // phase of the previous tick
       cudaStream_t S = T.s[parity];
       CK(cudaStreamWaitEvent(S, T.done[pp & 1], 0), "wait previous tick");
-      CK(launch_route(batch_params(bp, view(e, pp % 3), true), false, e->sm_count, S), "route_kernel");
-      if (bp->n) e->launches++;
+      const KParams P = batch_params(bp, view(e, pp % 3), true);
+      CK(launch_route(P, false, e->sm_count, S), "route_kernel");
+      e->launches += route_launches(P);
       T.prev = nullptr;
     }
     CK(cudaEventRecord(T.ev_join, T.s[1]), "join"); CK(cudaStreamWaitEvent(T.s[0], T.ev_join, 0), "join");
@@ -883,7 +898,8 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
       acc[0] = acc[1] = acc[2] = acc[3] = 0;
     }
   }
-  e->launches += (W ? refresh_launches(e) + (e->peers.ready && e->peers.world > 1 ? 1 : 0) : 0) + (bn->n ? 1 : 0) + (T.prev && T.prev->n ? 1 : 0);
+  e->launches += (W ? refresh_launches(e) + (e->peers.ready && e->peers.world > 1 ? 1 : 0) : 0) + (bn->n ? 1 : 0) +
+                 (T.prev ? route_launches(batch_params(T.prev, e->dt, true)) : 0);
   e->cur = phase % 3;   // the set this tick refreshed (a later plain dispatch continues from it)
   e->pools_dirty = false;
   bn->tick_no = T.n;
@@ -893,6 +909,32 @@ int tick_locked(cordum_engine* e, cordum_batch* bn, const cordum_worker_load* sl
   return CORDUM_OK;
 }
 int tick_flush_locked(cordum_engine* e) { return tick_locked(e, nullptr, nullptr, 0); }
+
+// The host encoder's selective list into the batch's pinned staging (grown on first need), for the next H2D of the records.
+int stage_selective(cordum_engine* e, cordum_batch* b) {
+  const auto &jobs = b->hr.sel_jobs, &extra = b->hr.sel_extra;
+  const size_t words = jobs.size() + extra.size();
+  if (words > b->sel_cap) {
+    std::lock_guard<std::mutex> g(e->mu);
+    CK(cudaSetDevice(e->device), "cudaSetDevice");
+    CK(cudaStreamSynchronize(b->stream), "wait before reallocating the selective list");
+    if (b->h_sel) cudaFreeHost(b->h_sel);
+    if (b->d_sel) cudaFree(b->d_sel);
+    b->h_sel = b->d_sel = nullptr; b->sel_cap = 0;
+    const size_t cap = std::max<size_t>(words + words / 4, 1024);
+    CK(cudaHostAlloc((void**)&b->h_sel, cap * 4, cudaHostAllocDefault), "pinned selective list");
+    CK(cudaMalloc((void**)&b->d_sel, cap * 4), "selective list");
+    b->sel_cap = cap;
+    e->tables_gen++;   // captured graphs bake the batch's pointers in
+  }
+  if (words) {
+    std::memcpy(b->h_sel, jobs.data(), jobs.size() * 4);
+    std::memcpy(b->h_sel + jobs.size(), extra.data(), extra.size() * 4);
+  }
+  b->n_sel_jobs = (uint32_t)(jobs.size() / 2);
+  b->sel_words = (uint32_t)words;
+  return CORDUM_OK;
+}
 
 int host_encode_into(cordum_engine* e, cordum_batch* b, const cordum_envelopes* env) {
   cordum::NvtxRange nvtx_("cordum:encode_host");
@@ -938,6 +980,7 @@ int host_encode_into(cordum_engine* e, cordum_batch* b, const cordum_envelopes* 
     if (rc != cordum::kWideRetry) break;   // the tables changed between the look and the encode: size again
   }
   if (rc) return rc == cordum::kWideRetry ? CORDUM_E_STALE : rc;
+  if (int rc2 = stage_selective(e, b)) return rc2;
   b->wide_words = b->hr.wide_words;
   b->epoch = epoch_before;
   b->encoded = true;
@@ -1353,6 +1396,7 @@ int32_t cordum_encode_device(cordum_engine* e, cordum_batch* b, const cordum_env
   b->n = n;
   b->encoded = false; b->resident = false; b->device_encoded = false;
   b->wide_words = 0;   // a batch the device encoder completes has none (wide tables raise the fallback flag)
+  b->n_sel_jobs = b->sel_words = 0;   // nor a selective list (a selective pair raises it too)
   if (n == 0) { b->encoded = true; b->resident = true; b->device_encoded = true; b->host_records_valid = true; b->epoch = e->host->epoch(); return CORDUM_OK; }
   if (!b->h_fallback) { CK(cudaHostAlloc((void**)&b->h_fallback, 64, cudaHostAllocDefault), "pinned flag"); *b->h_fallback = 0; }
   const uint32_t n_risk = env->risk_off ? env->risk_off[n] : 0, n_req = env->requires_off ? env->requires_off[n] : 0,

@@ -20,6 +20,7 @@ namespace cordum {
 namespace {
 
 constexpr uint32_t kMiss = 0xFFFFFFFFu;
+std::atomic<uint32_t> g_sel_min_bits{CORDUM_SEL_MIN_BITS}, g_sel_max_holders{CORDUM_SEL_MAX_HOLDERS};
 
 // fold_key without heap allocation for ordinary-sized ASCII values (anything else takes the general path)
 struct FoldBuf {
@@ -1239,6 +1240,11 @@ int Host::load_workers(const cordum_workers* w, std::string& err) {
   return CORDUM_OK;
 }
 
+void set_selective_limits(uint32_t min_bits, uint32_t max_holders) {
+  g_sel_min_bits = min_bits;
+  g_sel_max_holders = max_holders;
+}
+
 int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads) {
   HostTables& t = t_;
   auto& store = workers_raw_;
@@ -1262,24 +1268,55 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
   // placement-label dictionary: pairs (k,v!=""), per-key "absent or empty" bits, "has any label" bit
   uint32_t nbits = 0;
   const uint32_t any_bit = nbits++;
+  std::vector<uint32_t> pair_bits;   // the bits that stand for pairs, ascending
+  std::vector<uint32_t> holders;     // per bit: routable workers carrying the pair
   for (auto& p : pos)
     for (auto& kv : store[p.slot].labels) {
-      if (place_key.find(kv.first, kMiss) == kMiss) place_key.put(kv.first, nbits++);
+      if (place_key.find(kv.first, kMiss) == kMiss) { place_key.put(kv.first, nbits++); holders.push_back(0); }
       if (!kv.second.empty()) {
         const std::string pk = StrTable::pair_key(kv.first, kv.second);
-        if (place_pair.find(pk, kMiss) == kMiss) place_pair.put(pk, nbits++);
+        uint32_t b = place_pair.find(pk, kMiss);
+        if (b == kMiss) { b = nbits++; place_pair.put(pk, b); pair_bits.push_back(b); holders.push_back(0); }
+        holders[b - 1]++;   // holders[0] is bit 1: the "has any label" bit is no pair
       }
     }
-  {   // label bits beyond 128 spill into pos_label_x; what bounds them is the per-pool bitmaps (bits x workers / 8 bytes)
+  // Selective pairs (tables.h DeviceTables.sel_*): once the registry needs more placement bits than the limit, a pair
+  // carried by few routable workers (hostname-style labels) gets a holder list instead of a dense bit, a bitmap row per
+  // pool and a side-row bit per job.  The remaining bits keep their order and are renumbered densely.
+  const uint32_t sel_min_bits = g_sel_min_bits.load(), sel_max_holders = g_sel_max_holders.load();
+  std::vector<uint32_t> remap;   // old bit -> dense bit, or CORDUM_SEL_TAG | selective pair id (empty: nothing moves)
+  uint32_t dense_bits = nbits, n_sel = 0;
+  if (nbits > sel_min_bits) {
+    std::vector<uint8_t> sel(nbits, 0);
+    for (uint32_t b : pair_bits) sel[b] = holders[b - 1] <= sel_max_holders;
+    remap.resize(nbits);
+    dense_bits = 0;
+    for (uint32_t b = 0; b < nbits; ++b) remap[b] = sel[b] ? (CORDUM_SEL_TAG | n_sel++) : dense_bits++;
+    if (n_sel == 0) { remap.clear(); dense_bits = nbits; }
+  }
+  {   // label bits beyond 128 spill into pos_label_x; what bounds them is the per-pool bitmaps (dense bits x workers / 8 bytes)
     std::vector<uint32_t> per_pool(std::max<uint32_t>(t.n_pools, 1), 0);
     for (auto& p : pos) per_pool[p.pool]++;
     uint64_t words = 0;
-    for (uint32_t c : per_pool) words += (uint64_t)nbits * ((c + 31) / 32);
+    for (uint32_t c : per_pool) words += (uint64_t)dense_bits * ((c + 31) / 32);
     if (nbits > 65536 || words > (1ull << 31)) {
       err = "placement labels on routable workers need " + std::to_string(nbits) + " label bits and " + std::to_string(words * 4 >> 20) +
             " MiB of per-pool label bitmaps (limits: 65536 bits, 8 GiB)";
       return CORDUM_E_CAPACITY;
     }
+  }
+  if (!remap.empty()) {   // the dictionaries with the new numbering
+    StrTable pp, pk;
+    for (auto& p : pos)
+      for (auto& kv : store[p.slot].labels) {
+        if (!pk.contains(kv.first)) pk.put(kv.first, remap[place_key.find(kv.first, 0)]);
+        if (!kv.second.empty()) {
+          const std::string k = StrTable::pair_key(kv.first, kv.second);
+          if (!pp.contains(k)) pp.put(k, remap[place_pair.find(k, 0)]);
+        }
+      }
+    place_pair = std::move(pp);
+    place_key = std::move(pk);
   }
   // ---- phase 2: commit (cannot fail)
   t.n_slots = n;
@@ -1288,7 +1325,7 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
   place_pair_ = std::move(place_pair);
   place_key_ = std::move(place_key);
   place_any_bit_ = any_bit;
-  place_bits_ = nbits;
+  place_bits_ = dense_bits;
   t.rank_slot.assign(std::max<uint32_t>(n, 1), 0);
   for (uint32_t r = 0; r < live.size(); ++r) t.rank_slot[r] = live[r];
   const uint32_t np = (uint32_t)pos.size();
@@ -1296,7 +1333,7 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
   uint32_t cap = std::max<uint32_t>(np, 1);
   t.pos_pool.assign(cap, 0); t.pos_slot.assign(cap, 0); t.pos_rank.assign(cap, 0);
   t.pos_label_lo.assign(cap, 0); t.pos_label_hi.assign(cap, 0);
-  const uint32_t xp = nbits > 128 ? (nbits - 128 + 63) / 64 : 0;
+  const uint32_t xp = dense_bits > 128 ? (dense_bits - 128 + 63) / 64 : 0;
   t.wide.xw_place = xp;
   t.pos_label_x.assign((size_t)cap * xp + 1, 0);
   t.slot_pos.assign(std::max<uint32_t>(n, 1), 0);
@@ -1309,6 +1346,11 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
     for (auto& p : pos) for (auto& kv : store[p.slot].labels) if (seen.insert(kv.first).second)
       keys.emplace_back(kv.first, place_key_.find(kv.first, 0));
   }
+  // selective pairs: each worker's ids (pos_sel, CSR by pos) and each pair's holders (sel_pos, CSR by pair id)
+  t.n_sel = n_sel;
+  t.pos_sel_off.assign(cap + 1, 0);
+  t.pos_sel.clear();
+  t.sel_off.assign(n_sel + 1, 0);
   for (uint32_t i = 0; i < np; ++i) {
     const Pos& p = pos[i];
     t.pos_pool[i] = p.pool; t.pos_slot[i] = p.slot; t.pos_rank[i] = p.rank;
@@ -1319,17 +1361,30 @@ int Host::compile_workers(std::string& err, const std::vector<Load16>* new_loads
     uint64_t* mx = t.pos_label_x.data() + (size_t)i * xp;
     auto setb = [&](uint32_t b) { if (b < 128) m[b >> 6] |= 1ull << (b & 63); else mx[(b >> 6) - 2] |= 1ull << (b & 63); };
     const auto& labels = store[p.slot].labels;
+    const size_t s0 = t.pos_sel.size();
     if (!labels.empty()) {
       setb(place_any_bit_);
       for (auto& k : keys) {
         const std::string* val = nullptr;
         for (auto& kv : labels) if (kv.first == k.first) val = &kv.second;
-        if (!val || val->empty()) setb(k.second);   // labels[k] == "" (matchesLabels, :169-171)
-        else setb(place_pair_.find_pair(k.first, *val, 0));
+        if (!val || val->empty()) { setb(k.second); continue; }   // labels[k] == "" (matchesLabels, :169-171)
+        const uint32_t b = place_pair_.find_pair(k.first, *val, 0);
+        if (b & CORDUM_SEL_TAG) { t.pos_sel.push_back(b & ~CORDUM_SEL_TAG); t.sel_off[(b & ~CORDUM_SEL_TAG) + 1]++; }
+        else setb(b);
       }
     }
+    std::sort(t.pos_sel.begin() + s0, t.pos_sel.end());
+    t.pos_sel_off[i + 1] = (uint32_t)t.pos_sel.size();
     t.pos_label_lo[i] = m[0]; t.pos_label_hi[i] = m[1];
   }
+  for (uint32_t s = 0; s < n_sel; ++s) t.sel_off[s + 1] += t.sel_off[s];
+  t.sel_pos.assign(std::max<size_t>(t.pos_sel.size(), 1), 0);
+  {
+    std::vector<uint32_t> fill(t.sel_off.begin(), t.sel_off.end() - 1);
+    for (uint32_t i = 0; i < np; ++i)   // ascending pos: each pair's holders come out in pos order
+      for (uint32_t k = t.pos_sel_off[i]; k < t.pos_sel_off[i + 1]; ++k) t.sel_pos[fill[t.pos_sel[k]]++] = i;
+  }
+  if (t.pos_sel.empty()) t.pos_sel.push_back(0);
   for (uint32_t p = 0; p < t.n_pools; ++p) t.pool_off[p + 1] += t.pool_off[p];
   // per-pool label bitmaps (filled on the device by worker-table refresh kernels): place_bits rows of ceil(n/32) words
   t.place_bits = std::max<uint32_t>(place_bits_, 1);
@@ -1430,6 +1485,8 @@ struct EncodeCaches {
   static uint32_t lslot(sv k, sv v) {
     return (uint32_t)(((((uintptr_t)k.data() >> 1) ^ k.size()) * 0x9E3779B1u) ^ ((((uintptr_t)v.data() >> 1) ^ v.size()) * 0x85EBCA6Bu)) >> 22;
   }
+  // selective placement pairs: the ids of the job being encoded, and {slot, count, ids...} of this thread's JF_SELECTIVE jobs
+  std::vector<uint32_t> sel_ids, sel_rec;
 };
 
 namespace {
@@ -1515,7 +1572,8 @@ void Host::encode_job(const cordum_envelopes* env, uint32_t j, uint32_t tid, uin
   uint32_t flags = 0;
   jr.topic = tid;
   jr.orig = j;
-  jr.spare[0] = jr.spare[1] = 0;
+  jr.sel[0] = jr.sel[1] = 0;
+  cc.sel_ids.clear();
   flags |= topic_entries_[tid].flags;
   const bool has_meta = env->has_meta && env->has_meta[j];
   jr.tenant = (uint16_t)(ten & 0xFFFFu);   // resolved in pass 1 (resolve_tenant)
@@ -1597,7 +1655,11 @@ void Host::encode_job(const cordum_envelopes* env, uint32_t j, uint32_t tid, uin
   rr.req_pool = req_pool;
   // ---- labels: one pass
   uint64_t lab = label_empty_mask_, place[2] = {0, 0};
-  auto set_place = [&](uint32_t bit) { if (bit < 128) place[bit >> 6] |= 1ull << (bit & 63); else wx[o_place + (bit >> 6) - 2] |= 1ull << (bit & 63); };
+  auto set_place = [&](uint32_t bit) {
+    if (bit & CORDUM_SEL_TAG) cc.sel_ids.push_back(bit & ~CORDUM_SEL_TAG);   // a selective pair: no dense bit
+    else if (bit < 128) place[bit >> 6] |= 1ull << (bit & 63);
+    else wx[o_place + (bit >> 6) - 2] |= 1ull << (bit & 63);
+  };
   sv mcpv[12];
   sv secrets_label, pref_pool, pref_worker;
   bool have_secrets_label = false;
@@ -1654,6 +1716,16 @@ void Host::encode_job(const cordum_envelopes* env, uint32_t j, uint32_t tid, uin
   jr.lab = lab;
   rr.place_lo = place[0];
   rr.place_hi = place[1];
+  if (!cc.sel_ids.empty()) {
+    // route_kernel settles everything before the worker scan and leaves NO_WORKERS; route_select_kernel takes it from there.
+    // A pair nobody carries (JF_PLACE_UNSAT already) makes the job NO_WORKERS whatever else it names.
+    if (flags & JF_PLACE_UNSAT) cc.sel_ids.clear();
+    else {
+      flags |= JF_PLACE_UNSAT | JF_SELECTIVE;
+      jr.sel[0] = cc.sel_ids[0] + 1;
+      jr.sel[1] = cc.sel_ids.size() > 1 ? cc.sel_ids[1] + 1 : 0;
+    }
+  }
   // ---- MCP request (extractMCPRequest, kernel.go:395-414) and secrets (kernel.go:381-393)
   bool used = false;
   for (int f = 0; f < 4; ++f) {
@@ -1733,6 +1805,8 @@ int Host::encode_locked(const cordum_envelopes* env, HostRecords& out, std::stri
   const uint32_t n = env->n_jobs;
   const uint32_t ww = WIDE_WORDS(t_.wide);
   out.wide_words = ww;
+  out.sel_jobs.clear();
+  out.sel_extra.clear();
   if (n == 0) return CORDUM_OK;
   if (ww && (!out.wide || (uint64_t)n * ww > out.wide_cap)) { err = "wide-mask buffer missing or too small for this policy"; return kWideRetry; }
   const uint32_t nthreads = (n < 8192 || threads_ <= 1) ? 1u : threads_;
@@ -1742,6 +1816,7 @@ int Host::encode_locked(const cordum_envelopes* env, HostRecords& out, std::stri
   for (uint32_t i = 0; i < nthreads; ++i) {
     if (!caches[i]) caches[i] = std::make_unique<EncodeCaches>();
     caches[i]->gen = encode_gen_;
+    caches[i]->sel_rec.clear();
   }
   if (nthreads > 1 && !pool_) pool_ = std::make_unique<WorkPool>(threads_);
   static const bool trace = getenv("CORDUM_ENCODE_TRACE") != nullptr;
@@ -1813,6 +1888,12 @@ int Host::encode_locked(const cordum_envelopes* env, HostRecords& out, std::stri
         bool miss = false;
         encode_job(env, j, tid[j], ten[j], out.job[slot], out.route[slot], ww ? out.wide + (size_t)slot * ww : nullptr, miss, *caches[w]);
         if (miss) misses[w].push_back(j);
+        if (out.job[slot].flags & JF_SELECTIVE) {
+          auto& rec = caches[w]->sel_rec;
+          rec.push_back(slot);
+          rec.push_back((uint32_t)caches[w]->sel_ids.size());
+          rec.insert(rec.end(), caches[w]->sel_ids.begin(), caches[w]->sel_ids.end());
+        }
       }
     }
   };
@@ -1835,7 +1916,31 @@ int Host::encode_locked(const cordum_envelopes* env, HostRecords& out, std::stri
       const uint32_t slot = out.slot_of[j];
       encode_job(env, j, tid[j], ten[j], out.job[slot], out.route[slot], ww ? out.wide + (size_t)slot * ww : nullptr, miss, *caches[0]);
     }
+  gather_selective(out, nthreads);
   return CORDUM_OK;
+}
+
+// The batch's selective list (tables.h JobRecords) from the threads' records, in ascending slot order.
+void Host::gather_selective(HostRecords& out, uint32_t nthreads) const {
+  std::vector<std::pair<uint32_t, const uint32_t*>> jobs;   // slot, {slot, count, ids...}
+  for (uint32_t w = 0; w < nthreads; ++w) {
+    const auto& rec = caches_[w]->sel_rec;
+    for (size_t i = 0; i < rec.size(); i += 2 + rec[i + 1]) jobs.emplace_back(rec[i], rec.data() + i);
+  }
+  if (jobs.empty()) return;
+  std::sort(jobs.begin(), jobs.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  out.sel_jobs.reserve(2 * jobs.size());
+  out.sel_extra.assign(1, 0u);
+  for (const auto& [slot, r] : jobs) {
+    uint32_t x = 0;
+    if (r[1] > 2) {
+      x = (uint32_t)out.sel_extra.size();
+      out.sel_extra.push_back(r[1] - 2);
+      out.sel_extra.insert(out.sel_extra.end(), r + 4, r + 2 + r[1]);
+    }
+    out.sel_jobs.push_back(slot);
+    out.sel_jobs.push_back(x);
+  }
 }
 
 void Host::export_dicts(std::vector<uint8_t>& blob, EncodeTables& et) const {

@@ -276,6 +276,8 @@ struct HostTables {
   std::vector<uint32_t> pool_off, pos_pool, pos_slot, pos_rank, slot_pos, rank_slot, rank_pos, lbm_off;
   uint32_t place_bits = 1;
   uint64_t lbm_words = 0;
+  uint32_t n_sel = 0;                                          // selective placement pairs (tables.h DeviceTables.sel_*)
+  std::vector<uint32_t> sel_off, sel_pos, pos_sel_off, pos_sel;
   std::vector<uint32_t> chunk_pool, pool_chunk0, merge_list;   // worker-table refresh work list (tables.h)
   uint32_t n_chunks = 0, n_merge = 0, merge_smem = 0;
   std::vector<uint64_t> pos_label_lo, pos_label_hi;
@@ -295,7 +297,15 @@ struct HostRecords {
   uint64_t wide_cap = 0;         // 64-bit words available at `wide`
   uint32_t wide_words = 0;       // out: the row width the encode used
   uint64_t epoch = 0;            // out: the table epoch the ids belong to (read under the encoder's lock)
+  // out: the selective list (tables.h JobRecords): {slot, x} per JF_SELECTIVE job, then the extra words; both empty
+  // when no job of the batch names a selective pair
+  std::vector<uint32_t> sel_jobs, sel_extra;
 };
+
+// Which placement pairs are selective: registries with more than min_bits placement bits, pairs carried by at most
+// max_holders routable workers (CORDUM_SEL_MIN_BITS / CORDUM_SEL_MAX_HOLDERS).  Tests move both to run the dense and the
+// selective path on the same inputs; takes effect at the next worker / routing load.
+void set_selective_limits(uint32_t min_bits, uint32_t max_holders);
 
 // Persistent worker pool for the encoder: parallel_for over [0,n) in dynamically claimed chunks.  Completion
 // is "every item processed", not "every worker checked in": a worker the OS has descheduled (busy or
@@ -448,7 +458,7 @@ class Host {
   std::atomic<uint64_t> text_gen_{0};                   // generation of text_.back(), readable without the lock
   void publish_text();
   StrTable worker_slot_;      // worker_id -> slot (last wins)
-  StrTable place_pair_;       // StrTable::pair_key(key, value) -> bit   (value non-empty)
+  StrTable place_pair_;       // StrTable::pair_key(key, value) -> bit, or kSelTag | selective pair id   (value non-empty)
   StrTable place_key_;        // key -> bit E_k ("labels non-empty and k absent-or-empty")
   uint32_t place_any_bit_ = 0; // bit "worker has >= 1 label"
   uint32_t place_bits_ = 0;
@@ -468,6 +478,7 @@ class Host {
   uint32_t resolve_topic(const cordum_envelopes* env, uint32_t j, struct EncodeCaches& cc) const;   // kMiss = not in the dictionary
   uint32_t resolve_tenant(const cordum_envelopes* env, uint32_t j, struct EncodeCaches& cc) const;   // id | exact-policy index << 16
   void encode_job(const cordum_envelopes* env, uint32_t j, uint32_t tid, uint32_t ten, JobRec& jr, RouteRec& rr, uint64_t* wx, bool& miss, struct EncodeCaches& cc) const;
+  void gather_selective(HostRecords& out, uint32_t nthreads) const;
 };
 
 // test hooks (also exported through the C ABI as cordum_test_*)

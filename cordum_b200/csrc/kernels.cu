@@ -7,6 +7,8 @@
 //                        (engine.go:528-530)
 //   route_kernel         per job batch: pool filter + least-loaded pick (strategy_least_loaded.go:40-136) for the
 //                        jobs that may dispatch (engine.go:298-347)
+//   route_select_kernel  per job batch, after route_kernel: the worker pick of jobs that name selective placement pairs
+//                        (labels few workers carry, e.g. hostnames), from per-pair holder lists
 //
 // Integer / bit work only: no tensor cores (north star).  Mapping to the hardware:
 //   * a batch is two record arrays sorted by topic (64 B policy record, 32 B routing record per job).  A warp owns a
@@ -800,6 +802,102 @@ __global__ void __launch_bounds__(256, MINB) route_kernel(KParams P) {
   }
 }
 
+// ------------------------------------------------------------------ route: selective placement pairs
+// Jobs that name selective pairs (tables.h JF_SELECTIVE, DeviceTables.sel_*) carry JF_PLACE_UNSAT too, so route_kernel has
+// settled what the reference decides before its worker scan (:41-66) and left CORDUM_ROUTE_NO_WORKERS for the rest.  Runs
+// after route_kernel on the same stream, one warp per job of the batch's selective list:
+//   1  the eligible pools again (topic pool list or preferred pool, poolSatisfies)
+//   2  the preferred_worker_id shortcut (:73-87)
+//   3  the holders of the job's shortest selective list, one per lane; a holder is a candidate when its pool is eligible,
+//      its dense mask covers the dense needs and its own selective list holds the job's other selective needs (:161-175)
+//   4  candidate count and least-loaded pick over the non-overloaded ones, tie flag as route_kernel (:89-119, SURVEY A.4)
+__global__ void __launch_bounds__(256) route_select_kernel(KParams P) {
+  const DeviceTables& T = P.t;
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warps_total = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t item = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < P.recs.n_sel_jobs; item += warps_total) {
+    const uint2 ent = P.recs.sel_jobs[item];
+    const uint4* jr = reinterpret_cast<const uint4*>(P.recs.job + ent.x);
+    const uint4 a = __ldg(jr), sv = __ldg(jr + 3);   // {topic, flags, orig, ..}, {lab, sel[0], sel[1]}
+    const uint32_t flags = a.y;
+    uint32_t* o = reinterpret_cast<uint32_t*>(P.out + a.z);
+    const uint32_t h = o[0];   // written by route_kernel, earlier on this stream
+    if ((h >> 24) != CORDUM_ROUTE_NO_WORKERS || !(flags & JF_SELECTIVE)) continue;   // settled before the worker scan
+    const uint4 r0 = __ldg(reinterpret_cast<const uint4*>(P.recs.route + ent.x)), r1 = __ldg(reinterpret_cast<const uint4*>(P.recs.route + ent.x) + 1);
+    const uint64_t need_lo = ((uint64_t)r0.y << 32) | r0.x, need_hi = ((uint64_t)r0.w << 32) | r0.z;
+    const uint64_t need_req = (((uint64_t)r1.y << 32) | r1.x) & ~T.req_blank_mask;
+    const uint32_t ppool = r1.z, pwork = r1.w;
+    const uint64_t* wrow = (T.wide_words && P.recs.wide) ? P.recs.wide + (size_t)ent.x * T.wide_words : nullptr;
+    // the job's selective pair ids: sel[0], sel[1], then its extra words
+    const uint32_t n_ids = 1u + (sv.w ? 1u : 0u) + (ent.y ? __ldg(P.recs.sel_extra + ent.y) : 0u);
+    auto id_at = [&](uint32_t k) -> uint32_t { return k == 0 ? sv.z - 1u : k == 1 ? sv.w - 1u : __ldg(P.recs.sel_extra + ent.y + k - 1); };
+    // 1: pools.  A preferred pool passed route_kernel's check, so it is in the topic's list.
+    const uint32_t r_off = __ldg(T.topic_pool_off + a.x), r_cnt = __ldg(T.topic_pool_cnt + a.x);
+    const bool req_any = flags & JF_REQ_NONEMPTY, req_unknown = flags & JF_REQ_UNKNOWN;
+    auto pool_ok = [&](uint32_t pid) -> bool {   // poolSatisfies (:241-265) of a pool the job may use
+      bool listed = ppool ? pid == ppool - 1 : false;
+      for (uint32_t k = 0; !ppool && !listed && k < r_cnt; ++k) listed = __ldg(T.pool_list + r_off + k) == pid;
+      return listed && (!req_any || (__ldg(T.pool_req_nonempty + pid) && !req_unknown && pool_req_subset(T, pid, need_req, wrow)));
+    };
+    auto carries = [&](uint32_t pos, uint32_t skip) -> bool {   // matchesLabels (:161-175) but for selective need #skip
+      if ((__ldg(T.pos_label_lo + pos) & need_lo) != need_lo || (__ldg(T.pos_label_hi + pos) & need_hi) != need_hi || !place_x_ok(T, pos, wrow))
+        return false;
+      const uint32_t s0 = __ldg(T.pos_sel_off + pos), s1 = __ldg(T.pos_sel_off + pos + 1);
+      for (uint32_t k = 0; k < n_ids; ++k) {
+        if (k == skip) continue;
+        const uint32_t id = id_at(k);
+        bool found = false;
+        for (uint32_t q = s0; q < s1 && !found; ++q) found = __ldg(T.pos_sel + q) == id;
+        if (!found) return false;
+      }
+      return true;
+    };
+    uint32_t route = CORDUM_ROUTE_NO_WORKERS, rflags = 0;
+    int slot = -1;
+    // 2: preferred worker (every lane decides the same)
+    bool took_pref = false;
+    if (pwork && pwork != CORDUM_PREF_UNKNOWN) {
+      const uint32_t p1 = __ldg(T.slot_pos + (pwork - 1));
+      if (p1) {
+        const uint32_t pos = p1 - 1;
+        took_pref = pool_ok(__ldg(T.pos_pool + pos)) && carries(pos, 0xFFFFFFFFu) && !key_over(T.pos_key[pos]);
+      }
+    }
+    if (took_pref) { route = CORDUM_ROUTE_OK_PREFERRED; slot = (int)(pwork - 1); }
+    else {
+      // 3: the shortest holder list
+      uint32_t kmin = 0, len = 0xFFFFFFFFu;
+      for (uint32_t k = 0; k < n_ids; ++k) {
+        const uint32_t id = id_at(k), l = __ldg(T.sel_off + id + 1) - __ldg(T.sel_off + id);
+        if (l < len) { len = l; kmin = k; }
+      }
+      const uint32_t base = __ldg(T.sel_off + id_at(kmin));
+      uint64_t b = KEY_NONE;
+      uint32_t bc = 0, tot = 0;
+      for (uint32_t i = lane; i < len; i += 32) {
+        const uint32_t pos = __ldg(T.sel_pos + base + i);
+        if (!pool_ok(__ldg(T.pos_pool + pos)) || !carries(pos, kmin)) continue;
+        tot++;                                    // label-matching candidates, overloaded ones included
+        merge_best(b, bc, T.pos_key[pos], 1);     // merge_best skips overloaded keys
+      }
+      // 4: across the warp
+#pragma unroll
+      for (int off = 16; off; off >>= 1) {
+        const uint64_t k2 = shfl64_xor(FULL, b, off);
+        const uint32_t c2 = __shfl_xor_sync(FULL, bc, off);
+        merge_best(b, bc, k2, c2);
+        tot += __shfl_xor_sync(FULL, tot, off);
+      }
+      if (b != KEY_NONE) {
+        route = CORDUM_ROUTE_OK;
+        slot = (int)__ldg(T.rank_slot + (uint32_t)(b & 0xFFFFFFFFu));
+        if (bc > 1) rflags |= CORDUM_F_TIE;
+      } else route = tot > 0 ? CORDUM_ROUTE_POOL_OVERLOADED : CORDUM_ROUTE_NO_WORKERS;   // :114-119
+    }
+    if (lane == 0) { o[0] = (h & 0x00FFFFFFu) | (rflags << 16) | (route << 24); o[3] = (uint32_t)slot; }
+  }
+}
+
 // ------------------------------------------------------------------ heartbeat exchange over peer memory
 // One process per GPU; every rank owns a full slot-ordered load table (two alternate) that the other ranks have mapped
 // (CUDA IPC over NVLink / NVSwitch).  Per epoch a rank copies its own slice from the host into its table, PUSHES the slice
@@ -854,7 +952,7 @@ static cudaError_t configure_kernels() {
   const void* fns[] = {(const void*)worker_chunk_kernel<CORDUM_POOL_CHUNK>, (const void*)worker_merge_kernel, (const void*)peer_push_kernel,
                        (const void*)policy_kernel<3>, (const void*)policy_kernel<4>, (const void*)policy_kernel<5>, (const void*)policy_kernel<6>,
                        (const void*)route_kernel<true>, (const void*)route_kernel<false>,
-                       (const void*)route_kernel<false, 3>, (const void*)route_kernel<false, 5>};
+                       (const void*)route_kernel<false, 3>, (const void*)route_kernel<false, 5>, (const void*)route_select_kernel};
   for (const void* f : fns) {
     e = cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
@@ -921,5 +1019,12 @@ cudaError_t launch_route(const KParams& P, bool route_only, int sm_count, cudaSt
   else if (minb == 3) route_kernel<false, 3><<<blocks, 256, 0, s>>>(P);
   else if (minb == 5) route_kernel<false, 5><<<blocks, 256, 0, s>>>(P);
   else route_kernel<false><<<blocks, 256, 0, s>>>(P);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || route_launches(P) == 1) return e;
+  uint32_t sel_blocks = (P.recs.n_sel_jobs + 7u) / 8u;   // a warp per job
+  const uint32_t cap = (uint32_t)sm_count * 8u;
+  if (sel_blocks > cap) sel_blocks = cap;
+  if (share > 0 && sel_blocks > (uint32_t)(sm_count * share)) sel_blocks = (uint32_t)(sm_count * share);
+  route_select_kernel<<<sel_blocks, 256, 0, s>>>(P);
   return cudaGetLastError();
 }

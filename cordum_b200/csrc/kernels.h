@@ -32,7 +32,9 @@ cudaError_t launch_configure();
 // loads_read (optional) is recorded once T.loads has been consumed (between the chunk and the merge kernel)
 cudaError_t launch_worker_pools(const DeviceTables& T, cudaStream_t s, cudaEvent_t loads_read);   // chunk sort, merge, label_best
 cudaError_t launch_policy(const KParams& P, int sm_count, cudaStream_t s, int share = 0);
+// route_kernel, then route_select_kernel when the tables hold selective pairs and the batch lists jobs that name them
 cudaError_t launch_route(const KParams& P, bool route_only, int sm_count, cudaStream_t s, int share = 0);
+inline uint32_t route_launches(const KParams& P) { return P.n_jobs ? 1u + (P.t.n_sel && P.recs.n_sel_jobs ? 1u : 0u) : 0u; }
 
 // ---- device-side encoder (encode.cu)
 struct EncodeParams {

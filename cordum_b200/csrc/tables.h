@@ -17,6 +17,7 @@
 #include <vector_types.h>
 #else
 typedef struct __attribute__((aligned(16))) uint4 { unsigned int x, y, z, w; } uint4;
+typedef struct __attribute__((aligned(8))) uint2 { unsigned int x, y; } uint2;
 #endif
 
 /* 16-byte units (the kernels reinterpret these as uint4 / int4) */
@@ -48,6 +49,9 @@ typedef struct __attribute__((aligned(16))) Load16 { int32_t active, max_paralle
                                            requires list fails containsAll (safety_policy.go:320-330)            */
 #define JF_NO_LAB 0x8000u               /* no labels, or none of the label pairs any rule lists: every rule with a
                                            labels map fails labelsMatch (safety_policy.go:332-345)               */
+#define JF_SELECTIVE 0x10000u           /* the job needs selective placement pairs (DeviceTables.sel_*): JobRec.sel holds the
+                                           first two (id + 1), the batch's selective list the rest; JF_PLACE_UNSAT is set
+                                           too, so route_kernel leaves CORDUM_ROUTE_NO_WORKERS for route_select_kernel     */
 /* row_combo index: actor_type / secrets_present combination + 6 * NO_REQ + 12 * NO_LAB (24 rows) */
 #define CORDUM_COMBO_ROWS 24u
 #define CORDUM_COMBO_INDEX(flags) (((flags) & JF_COMBO_MASK) + (((flags) >> 14) & 3u) * 6u)
@@ -77,7 +81,7 @@ typedef struct __attribute__((aligned(16))) JobRec {   /* 64 B: everything polic
   uint64_t risk;         /* bit per referenced risk tag                                                */
   uint64_t req;          /* bit per referenced requires token, EqualFold canonical (rules' containsAll) */
   uint64_t lab;          /* bit per rule label pair (k,v): labels.get(k,"") == v                       */
-  uint32_t spare[2];
+  uint32_t sel[2];       /* JF_SELECTIVE: the job's first two selective pair ids + 1 (0 = none)        */
 } JobRec;
 typedef struct __attribute__((aligned(16))) RouteRec {   /* 32 B: what only route_kernel reads */
   uint64_t place_lo, place_hi;   /* placement need mask                                                */
@@ -97,6 +101,7 @@ enum {
   DD_TOPIC = 0, DD_TENANT, DD_TENANT_POL, DD_CAP, DD_PACK, DD_ACTOR, DD_RISK, DD_REQ, DD_MCP0, DD_MCP1, DD_MCP2, DD_MCP3,
   DD_LABEL_KEY, DD_LABEL_PAIR, DD_PLACE_PAIR, DD_PLACE_KEY, DD_POOL, DD_WORKER, DD_EFFCFG, DD_COUNT
 };
+#define CORDUM_SEL_TAG 0x80000000u      /* DD_PLACE_PAIR value of a selective pair: CORDUM_SEL_TAG | pair id (else: dense bit) */
 typedef struct EncodeTables {
   const uint8_t* blob;            /* device: all dictionaries                                             */
   DevDict dict[DD_COUNT];
@@ -110,16 +115,24 @@ typedef struct EncodeTables {
   uint32_t wide_words;            /* != 0: the device encoder hands the whole batch to the host encoder            */
 } EncodeTables;
 
+/* A batch's selective list (jobs flagged JF_SELECTIVE), one array of 32-bit words:
+     [n_sel_jobs x {slot j in the sorted records, x}] [extra words]
+   x = 0: the job names at most two selective pairs (JobRec.sel); else extra[x] = c, extra[x+1 .. x+c] = its further pair
+   ids (extra[0] is a 0 word, so x = 0 never points at a list).  Entries are in ascending j. */
 typedef struct JobRecords {
   const JobRec* job;
   const RouteRec* route;
   const uint64_t* wide;   /* [n_jobs][DeviceTables.wide_words], same (sorted) order; NULL when wide_words == 0 */
+  const uint2* sel_jobs;  /* the selective list (NULL when n_sel_jobs == 0)                                   */
+  const uint32_t* sel_extra;
+  uint32_t n_sel_jobs;
 } JobRecords;
 
 /* Wide masks.  The records hold 64 bits per mask (placement: 128).  A policy that references more than 64 distinct risk
-   tags / requires tokens / label pairs, or a registry with more than 128 placement-label bits, spills the further bits into
-   a side row of 64-bit words per job: [risk xw_risk][requires, EqualFold form xw_req][label pairs xw_lab]
-   [requires, ToLower form xw_req][placement xw_place].  All xw_* are 0 in the common case and nothing of this is read. */
+   tags / requires tokens / label pairs, or a registry with more than 128 dense placement-label bits, spills the further
+   bits into a side row of 64-bit words per job: [risk xw_risk][requires, EqualFold form xw_req][label pairs xw_lab]
+   [requires, ToLower form xw_req][placement xw_place].  All xw_* are 0 in the common case and nothing of this is read.
+   Selective placement pairs (DeviceTables.sel_*) take no bit here. */
 typedef struct WideLayout {
   uint32_t xw_risk, xw_req, xw_lab, xw_place;
 } WideLayout;
@@ -133,6 +146,8 @@ typedef struct WideLayout {
 #define CORDUM_POOL_CHUNK 512u
 #define CORDUM_POOL_SORT_MAX 8192u
 #define CORDUM_LBEST_MAX_BITS 1024u
+#define CORDUM_SEL_MIN_BITS CORDUM_LBEST_MAX_BITS   /* selective pairs only in registries with more placement bits than this */
+#define CORDUM_SEL_MAX_HOLDERS 32u                  /* a selective pair is carried by at most this many routable workers     */
 
 typedef struct DeviceTables {
   /* ---- policy.  All pass-row tables live in ONE word-major array on the device: the 16 B cell of word w for value v of
@@ -192,7 +207,15 @@ typedef struct DeviceTables {
   uint4* lbest;                               /* derived, or NULL (place_bits > CORDUM_LBEST_MAX_BITS): per (pool, label bit) what a
                                                  job that requires exactly that one label gets from the pool's sorted view -
                                                  {key lo, key hi (KEY_NONE: nobody), 1 | 2 = tie inside the pool, matching workers}  */
-  uint32_t place_bits;                        /* label bits in use (beyond 128: pos_label_x)                               */
+  uint32_t place_bits;                        /* dense label bits in use (beyond 128: pos_label_x)                         */
+  /* selective placement pairs: pairs (k, v != "") carried by at most CORDUM_SEL_MAX_HOLDERS routable workers, in a registry
+     whose placement labels need more than CORDUM_SEL_MIN_BITS bits.  They have no dense bit, bitmap row or lbest row:
+     route_select_kernel finds a job's candidates through the holder lists instead.                                    */
+  uint32_t n_sel;                             /* selective pairs (0: none, route_select_kernel is never launched)          */
+  const uint32_t* sel_off;                    /* [n_sel+1] range of the pair in sel_pos                                    */
+  const uint32_t* sel_pos;                    /* pos of every routable worker carrying the pair, ascending per pair         */
+  const uint32_t* pos_sel_off;                /* [n_pos+1] range of the worker in pos_sel                                  */
+  const uint32_t* pos_sel;                    /* selective pair ids the worker carries, ascending per worker                */
   /* worker-table refresh: a pool is cut into chunks of CORDUM_POOL_CHUNK workers, one CTA sorts one chunk, a second
      kernel merges the chunks of pools that have more than one (pools above CORDUM_POOL_SORT_MAX stay unsorted)       */
   const uint32_t* chunk_pool;                 /* [n_chunks] pool of the chunk                                              */

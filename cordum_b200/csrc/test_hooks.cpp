@@ -6,6 +6,7 @@
 // the tables in Python the way kernels.cu does).  They evaluate nothing themselves.
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "host.hpp"
 
@@ -16,6 +17,7 @@ using cordum::sv;
 
 namespace {
 thread_local std::string t_err;
+thread_local std::vector<uint32_t> t_sel_jobs, t_sel_extra;   // the selective list of the last cordum_test_host_encode
 }  // namespace
 
 extern "C" {
@@ -49,8 +51,22 @@ int32_t cordum_test_host_encode(void* h, const cordum_envelopes* env, uint8_t* s
   r.job = (JobRec*)slab;
   r.route = (RouteRec*)(slab + (size_t)n * sizeof(JobRec));
   r.slot_of = (uint32_t*)(slab + (size_t)n * (sizeof(JobRec) + sizeof(RouteRec)));
-  return ((Host*)h)->encode(env, r, t_err);
+  const int32_t rc = ((Host*)h)->encode(env, r, t_err);
+  t_sel_jobs = std::move(r.sel_jobs);
+  t_sel_extra = std::move(r.sel_extra);
+  return rc;
 }
+// the selective list (tables.h JobRecords) of the last cordum_test_host_encode on this thread: which = 0 the {slot, x}
+// pairs, 1 the extra words
+int32_t cordum_test_host_sel(int32_t which, const void** ptr, uint64_t* bytes) {
+  const std::vector<uint32_t>& v = which ? t_sel_extra : t_sel_jobs;
+  *ptr = v.data();
+  *bytes = v.size() * sizeof(uint32_t);
+  return 0;
+}
+// selective placement pairs in registries above min_bits placement bits, for pairs with at most max_holders routable
+// holders (defaults CORDUM_SEL_MIN_BITS, CORDUM_SEL_MAX_HOLDERS); process-wide, from the next worker / routing load on
+void cordum_test_set_selective(uint32_t min_bits, uint32_t max_holders) { cordum::set_selective_limits(min_bits, max_holders); }
 
 // common/mini_json.hpp (shared by the product and the oracle) differentially against an independent parser:
 // returns -1 when the document is rejected, else the length of the re-dumped tree (written to buf up to cap)
@@ -82,6 +98,7 @@ int32_t cordum_test_host_table(void* h, const char* name, const void** ptr, uint
   VEC("pool_off", t.pool_off) VEC("pos_pool", t.pos_pool) VEC("pos_slot", t.pos_slot) VEC("pos_rank", t.pos_rank)
   VEC("slot_pos", t.slot_pos) VEC("rank_slot", t.rank_slot) VEC("pos_label_lo", t.pos_label_lo)
   VEC("pos_label_hi", t.pos_label_hi) VEC("loads", t.loads)
+  VEC("sel_off", t.sel_off) VEC("sel_pos", t.sel_pos) VEC("pos_sel_off", t.pos_sel_off) VEC("pos_sel", t.pos_sel)
   VEC("chunk_pool", t.chunk_pool) VEC("pool_chunk0", t.pool_chunk0) VEC("merge_list", t.merge_list)
   VEC("tenant_class", ((Host*)h)->tenant_class())
 #undef VEC
@@ -114,6 +131,8 @@ uint64_t cordum_test_host_scalar(void* h, const char* name) {
   if (n == "xw_lab") return t.wide.xw_lab;
   if (n == "xw_place") return t.wide.xw_place;
   if (n == "place_bits") return t.place_bits;
+  if (n == "n_sel") return t.n_sel;
+  if (n == "lbm_words") return t.lbm_words;
   return ~0ull;
 }
 

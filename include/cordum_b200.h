@@ -33,7 +33,10 @@ extern "C" {
 /* ---------------------------------------------------------------- status */
 #define CORDUM_OK 0
 #define CORDUM_E_INVALID (-1)   /* bad argument / malformed input document        */
-#define CORDUM_E_CAPACITY (-2)  /* a dictionary exceeded its mask width (64)      */
+#define CORDUM_E_CAPACITY (-2)  /* a table outgrew its bound: 65,535 values per dictionary, 65,536 placement-label keys +
+                                   pairs per registry, 8 GiB of label bitmaps (dense bits only: pairs carried by <= 32
+                                   workers in registries above 1,024 label bits have none), 4 GiB of wide-mask rows per
+                                   batch; the previous tables stay in force */
 #define CORDUM_E_CUDA (-3)      /* CUDA runtime / kernel failure (sticky)         */
 #define CORDUM_E_STATE (-4)     /* call order violated (e.g. dispatch before load)*/
 #define CORDUM_E_NODEVICE (-5)  /* no CUDA device: the product has NO CPU path    */
@@ -296,7 +299,9 @@ int32_t cordum_encode(cordum_engine* e, cordum_batch* b, const cordum_envelopes*
  * unchanged until cordum_batch_wait returns.  Page-locked buffers (cordum_envelopes_alloc) are copied by DMA at full
  * PCIe rate; pageable memory works too, slower.
  * What the device leaves to the host - first sight of a topic or of an effective config (pass-rows have to be
- * computed / JSON parsed), non-ASCII text (Unicode TrimSpace / EqualFold), strings over 4 KiB - raises a per-batch
+ * computed / JSON parsed), non-ASCII text (Unicode TrimSpace / EqualFold), strings over 4 KiB, masks wider than the
+ * records (more than 64 referenced risk tags / requires tokens / rule label pairs, more than 128 dense placement-label
+ * bits), a placement label few workers carry (a selective pair, e.g. a hostname, in a registry above 1,024 label bits) - raises a per-batch
  * flag; cordum_batch_wait then encodes that batch with cordum_encode's code path and runs it again, so results are
  * the same either way (tests compare the two encoders record for record). */
 typedef struct cordum_envelope_caps {
