@@ -173,6 +173,10 @@ struct cordum_batch {
   uint64_t tick_no = 0;          // the tick it was handed in with (its route runs in tick_no + 1)
   cordum_decision* h_out = nullptr;   // pinned
   cordum_decision* d_out = nullptr;
+  bool results_ready = false;    // d_out holds the complete records of the last dispatch (cordum_batch_plan reads them)
+  DevBuf d_plan;                 // cordum_batch_plan scratch (plan_batch), grown on first need
+  uint32_t* h_plan = nullptr;    // pinned: the plan's offsets, the record-check flag, then its jobs
+  size_t h_plan_cap = 0;         // 32-bit words
   uint2* d_route = nullptr;           // [0].x = count, [2..] = compacted list of dispatchable jobs {slot, head}
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, ev2 = nullptr, ev3 = nullptr;
@@ -519,6 +523,7 @@ int run(cordum_engine* e, cordum_batch* b, uint32_t mode, bool copy_in, bool cop
   if (b->device_encoded) copy_in = false;   // the records were produced on the device
   if (!copy_in && !b->resident) { g_err = "batch columns are not resident on the device"; return CORDUM_E_STATE; }
   b->last_mode = mode | (flush_l2 ? CORDUM_FLAG_FLUSH_L2 : 0u) | (timed ? 0u : CORDUM_FLAG_NO_TIMING);
+  b->results_ready = false;
   b->timed = timed;
   b->last_copy_out = copy_out;
   if (b->pending) { CK(cudaStreamSynchronize(b->stream), "wait previous"); b->pending = false; b->enc_inflight = false; }
@@ -592,6 +597,7 @@ int wait(cordum_batch* b) {
     }
     for (cudaStream_t st : e->tick.s) CK(cudaStreamSynchronize(st), "tick wait");
     b->tick_pending = false;
+    b->results_ready = true;
     b->total_ms = b->kernel_ms = b->policy_ms = b->route_ms = 0;
   }
   if (!b->pending && !b->enc_inflight) return CORDUM_OK;
@@ -613,6 +619,7 @@ int wait(cordum_batch* b) {
     b->pending = false;
   }
   if (!dispatched) return CORDUM_OK;
+  b->results_ready = true;
   if (!b->timed) { b->total_ms = b->kernel_ms = b->policy_ms = b->route_ms = 0; return CORDUM_OK; }
   CK(cudaEventElapsedTime(&b->total_ms, b->timed_in ? b->ev0 : b->ev1, b->timed_out ? b->ev3 : b->ev2), "elapsed");
   CK(cudaEventElapsedTime(&b->kernel_ms, b->ev1, b->ev2), "elapsed");
@@ -641,6 +648,7 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->h_sel) cudaFreeHost(b->h_sel);
   if (b->d_sel) cudaFree(b->d_sel);
   if (b->h_out) cudaFreeHost(b->h_out);
+  if (b->h_plan) cudaFreeHost(b->h_plan);
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
   std::free(b->slot_of);
@@ -943,6 +951,7 @@ int host_encode_into(cordum_engine* e, cordum_batch* b, const cordum_envelopes* 
   b->encoded = false;
   b->resident = false;
   b->device_encoded = false;
+  b->results_ready = false;
   uint64_t epoch_before = 0;
   int rc = CORDUM_OK;
   for (int attempt = 0; attempt < 3; ++attempt) {
@@ -985,6 +994,61 @@ int host_encode_into(cordum_engine* e, cordum_batch* b, const cordum_envelopes* 
   b->epoch = epoch_before;
   b->encoded = true;
   b->host_records_valid = true;
+  return CORDUM_OK;
+}
+
+// cordum_batch_plan on a batch whose records are complete in d_out.  Device scratch (32-bit words): keys / values x 2 (n
+// each) | counts [256][tiles] | totals [256] | offsets [n_buckets + 1] | flag; pinned: offsets | flag | jobs [n].
+int plan_batch(cordum_engine* e, cordum_batch* b, cordum_plan* out) {
+  PlanParams P{};
+  P.recs = b->d_out;
+  P.n = b->n;
+  P.n_slots = b->wtext ? (uint32_t)b->wtext->size() : 0u;   // the registry the batch was routed on
+  P.n_buckets = P.n_slots + CORDUM_PLAN_OUTCOMES;
+  const size_t n = P.n, nb = P.n_buckets, tiles = (n + CORDUM_PLAN_TILE - 1) / CORDUM_PLAN_TILE;
+  const size_t dev_words = n ? 4 * n + 256 * tiles + 256 + nb + 2 : 0, host_words = nb + 2 + n;
+  if (dev_words * 4 > b->d_plan.cap || host_words > b->h_plan_cap) {
+    // an allocation that does not fit is this call's problem, not a sticky engine failure
+    const size_t dev_bytes = dev_words * 4;
+    const cudaError_t de = dev_bytes > b->d_plan.cap ? b->d_plan.reserve(dev_bytes + dev_bytes / 4) : cudaSuccess;
+    cudaError_t he = cudaSuccess;
+    if (de == cudaSuccess && host_words > b->h_plan_cap) {
+      if (b->h_plan) cudaFreeHost(b->h_plan);
+      b->h_plan = nullptr; b->h_plan_cap = 0;
+      const size_t want = host_words + host_words / 4;
+      he = cudaHostAlloc((void**)&b->h_plan, want * 4, cudaHostAllocDefault);
+      if (he == cudaSuccess) b->h_plan_cap = want;
+      else b->h_plan = nullptr;
+    }
+    if (de != cudaSuccess || he != cudaSuccess) {
+      cudaGetLastError();
+      g_err = "out of memory for the plan of " + std::to_string(n) + " jobs over " + std::to_string(nb) + " buckets";
+      return CORDUM_E_CAPACITY;
+    }
+  }
+  uint32_t* h = b->h_plan;
+  out->n_slots = P.n_slots;
+  out->n_jobs = P.n;
+  out->offsets = h;
+  out->jobs = h + nb + 2;
+  if (n == 0) { std::memset(h, 0, (nb + 1) * 4); return CORDUM_OK; }
+  uint32_t* w = (uint32_t*)b->d_plan.p;
+  P.keys[0] = w; P.vals[0] = w + n; P.keys[1] = w + 2 * n; P.vals[1] = w + 3 * n;
+  P.counts = w + 4 * n;
+  P.totals = P.counts + 256 * tiles;
+  P.offsets = P.totals + 256;
+  P.bad = P.offsets + nb + 1;
+  cudaStream_t s = b->stream;
+  CK(launch_plan(P, s), "plan kernels");
+  e->launches += plan_launches(P);
+  CK(cudaMemcpyAsync(h, P.offsets, (nb + 2) * 4, cudaMemcpyDeviceToHost, s), "D2H plan offsets");
+  CK(cudaMemcpyAsync(h + nb + 2, P.vals[(plan_passes(P.n_buckets) - 1) & 1], n * 4, cudaMemcpyDeviceToHost, s), "D2H plan jobs");
+  CK(cudaStreamSynchronize(s), "plan");
+  if (h[nb + 1]) {
+    g_err = "a decision record of this batch names a worker slot outside the registry it was dispatched against (the registry "
+            "was reloaded while the batch was in flight): encode and dispatch it again";
+    return CORDUM_E_STALE;
+  }
   return CORDUM_OK;
 }
 }  // namespace
@@ -1247,6 +1311,7 @@ int32_t cordum_tick_async(cordum_engine* e, cordum_batch* b, uint32_t mode, cons
   std::lock_guard<std::mutex> gh(e->host->mutex());
   if (b->epoch != e->host->epoch()) { g_err = "tables were reloaded after this batch was encoded: encode again"; return CORDUM_E_STALE; }
   b->text = e->host->policy_text(); b->wtext = e->host->worker_text(); b->ttext = e->host->topic_text();
+  b->results_ready = false;
   const uint32_t W = e->host->tables().n_slots;
   if (e->peers.ready && e->peers.world > 1) {
     if (first_slot != (uint32_t)e->peers.rank * e->peers.per || n_slice != e->peers.per || e->peers.per * (uint32_t)e->peers.world != W) {
@@ -1394,7 +1459,7 @@ int32_t cordum_encode_device(cordum_engine* e, cordum_batch* b, const cordum_env
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   const uint32_t n = env->n_jobs;
   b->n = n;
-  b->encoded = false; b->resident = false; b->device_encoded = false;
+  b->encoded = false; b->resident = false; b->device_encoded = false; b->results_ready = false;
   b->wide_words = 0;   // a batch the device encoder completes has none (wide tables raise the fallback flag)
   b->n_sel_jobs = b->sel_words = 0;   // nor a selective list (a selective pair raises it too)
   if (n == 0) { b->encoded = true; b->resident = true; b->device_encoded = true; b->host_records_valid = true; b->epoch = e->host->epoch(); return CORDUM_OK; }
@@ -1520,6 +1585,15 @@ int32_t cordum_batch_kernel_times(const cordum_batch* b, float* policy_ms, float
   if (policy_ms) *policy_ms = b->policy_ms;
   if (route_ms) *route_ms = b->route_ms;
   return CORDUM_OK;
+}
+int32_t cordum_batch_plan(cordum_batch* b, cordum_plan* out) {
+  cordum::NvtxRange nvtx_("cordum:plan");
+  if (!b || !out) { g_err = "null argument"; return CORDUM_E_INVALID; }
+  cordum_engine* e = b->e;
+  if (e->failed) { g_err = "engine failed earlier: " + e->fail_msg; return CORDUM_E_CUDA; }
+  if (!b->results_ready) { g_err = "the batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first"; return CORDUM_E_STATE; }
+  CK(cudaSetDevice(e->device), "cudaSetDevice");
+  return plan_batch(e, b, out);
 }
 /* copies the decision records still on the device into the pinned result buffer (after a resident run) */
 int32_t cordum_batch_fetch(cordum_batch* b) {

@@ -36,6 +36,29 @@ cudaError_t launch_policy(const KParams& P, int sm_count, cudaStream_t s, int sh
 cudaError_t launch_route(const KParams& P, bool route_only, int sm_count, cudaStream_t s, int share = 0);
 inline uint32_t route_launches(const KParams& P) { return P.n_jobs ? 1u + (P.t.n_sel && P.recs.n_sel_jobs ? 1u : 0u) : 0u; }
 
+// ---- batch dispatch plan (plan.cu): the jobs of a batch grouped by bucket key (include/cordum_b200.h cordum_plan)
+#define CORDUM_PLAN_TILE 2048u   // jobs per CTA of the count / scatter kernels
+struct PlanPass {                // one 8-bit radix pass
+  const uint4* recs;             // pass 0: the decision records (keys are derived from them); later passes: null
+  const uint32_t *keys_in, *vals_in;
+  uint32_t *keys_out, *vals_out;
+  uint32_t* counts;              // [256][n_tiles]
+  uint32_t* totals;              // [256]
+  uint32_t* bad;                 // raised when a record fits no bucket
+  uint32_t n, n_slots, n_tiles, shift;
+};
+struct PlanParams {
+  const cordum_decision* recs;   // device, n records in caller order
+  uint32_t n, n_slots, n_buckets;
+  uint32_t *keys[2], *vals[2];   // device scratch, n each: the passes alternate between them
+  uint32_t *counts, *totals, *bad;
+  uint32_t* offsets;             // device, n_buckets + 1
+};
+uint32_t plan_passes(uint32_t n_buckets);
+// The sorted job indices end in vals[(plan_passes(n_buckets) - 1) & 1].
+cudaError_t launch_plan(const PlanParams& P, cudaStream_t s);
+inline uint32_t plan_launches(const PlanParams& P) { return P.n ? 3u * plan_passes(P.n_buckets) + 1u : 0u; }
+
 // ---- device-side encoder (encode.cu)
 struct EncodeParams {
   uint32_t n_jobs;

@@ -119,6 +119,26 @@ class Batch:
         self.eng._ck(self.L.cordum_batch_kernel_times(self.h, C.byref(p), C.byref(r)))
         return p.value, r.value
 
+    def plan(self):
+        """(offsets, jobs, n_slots) of the last completed dispatch (cordum_batch_plan): jobs grouped by destination worker
+        slot (buckets 0 .. n_slots-1), then by outcome (bucket n_slots + k, wire.PLAN_OUTCOME_NAMES[k]); bucket b holds
+        jobs[offsets[b]:offsets[b+1]], ascending.  Views of library memory, valid until this batch's next encode,
+        dispatch, plan or free."""
+        p = wire.CordumPlan()
+        self.eng._ck(self.L.cordum_batch_plan(self.h, C.byref(p)))
+        nb = p.n_slots + wire.PLAN_OUTCOMES
+
+        def view(ptr, count):
+            return np.frombuffer((C.c_uint32 * count).from_address(ptr), dtype=np.uint32, count=count) if count else np.zeros(0, np.uint32)
+
+        return view(p.offsets, nb + 1), view(p.jobs, p.n_jobs), int(p.n_slots)
+
+    @staticmethod
+    def plan_buckets(offsets, jobs):
+        """The non-empty buckets of a plan: (bucket, job indices) pairs in bucket order."""
+        for b in np.flatnonzero(np.diff(offsets)):
+            yield int(b), jobs[offsets[b]:offsets[b + 1]]
+
     def _text(self, fn, job: int, *extra) -> str:
         buf = C.create_string_buffer(4096)
         n = fn(self.eng.h, self.h, job, *extra, buf, len(buf))

@@ -118,6 +118,11 @@ class CordumTableStats(C.Structure):
     ]
 
 
+class CordumPlan(C.Structure):
+    """cordum_plan: a dispatched batch's jobs grouped by destination worker slot, then by outcome (cordum_batch_plan)."""
+    _fields_ = [("n_slots", C.c_uint32), ("n_jobs", C.c_uint32), ("offsets", C.c_void_p), ("jobs", C.c_void_p)]
+
+
 class CordumEnvelopeCaps(C.Structure):
     _fields_ = [("max_jobs", C.c_uint32), ("max_risk_tags", C.c_uint32), ("max_requires", C.c_uint32), ("max_labels", C.c_uint32),
                 ("arena_bytes", C.c_uint64)]
@@ -144,6 +149,9 @@ MODE_POLICY_ONLY, MODE_POLICY_AND_ROUTE, MODE_ROUTE_ONLY = 1, 2, 3
 FLAG_FLUSH_L2 = 0x100
 REASON_FLAVOR_KERNEL, REASON_FLAVOR_GATEWAY = 0, 1   # cordum_reason_flavor
 FLAG_NO_TIMING = 0x200
+# dispatch plan: bucket n_slots + k holds the jobs of outcome k (include/cordum_b200.h CORDUM_PLAN_*)
+PLAN_OUTCOMES = 12
+PLAN_OUTCOME_NAMES = DEC_NAMES + ["MISSING_TOPIC", "NO_POOL_PREFERRED", "NO_POOL_TOPIC", "NO_POOL_REQUIRES", "NO_WORKERS", "POOL_OVERLOADED"]
 REASON_NONE, REASON_RULE, REASON_MISSING_TOPIC, REASON_UNSUPPORTED_TOPIC, REASON_TENANT_MCP = 0, 1, 2, 3, 4
 REASON_EFF_DENIED_TOPIC, REASON_EFF_NOT_ALLOWED_TOPIC, REASON_EFF_MCP, REASON_APPROVAL_GRANTED = 12, 13, 14, 22
 

@@ -345,6 +345,42 @@ int32_t cordum_batch_timing(const cordum_batch* b, float* total_ms, float* kerne
 /* The two kernels of a dispatch separately: policy_kernel and route_kernel (CUDA events). */
 int32_t cordum_batch_kernel_times(const cordum_batch* b, float* policy_ms, float* route_ms);
 
+/* ---- dispatch plan: the jobs of a dispatched batch grouped by what processJob does with them (engine.go:298-347,
+ * 393-442), computed on the device from the decision records, so that a bulk caller need not fetch 16 B per job and
+ * group them itself.  Buckets 0 .. n_slots-1: the jobs routed (ROUTE_OK / OK_PREFERRED) to that worker slot, published to
+ * cordum_subject's "worker.<id>.jobs".  Bucket n_slots + k: every other job, by outcome k: */
+#define CORDUM_PLAN_OUTCOMES 12
+#define CORDUM_PLAN_UNSPECIFIED 0        /* not routed, sched_decision UNSPECIFIED: "denied (unknown decision)", DLQ (engine.go:336-346) */
+#define CORDUM_PLAN_ALLOW 1              /* not routed (POLICY_ONLY), ALLOW: may dispatch (engine.go:299-302)                */
+#define CORDUM_PLAN_DENY 2               /* DENY: job denied, DLQ "safety_denied", safety_denied counter (engine.go:325-335)  */
+#define CORDUM_PLAN_REQUIRE_HUMAN 3      /* REQUIRE_HUMAN: job state APPROVAL, awaits a human (engine.go:316-324)             */
+#define CORDUM_PLAN_THROTTLE 4           /* THROTTLE: RetryAfter(safetyThrottleDelay) (engine.go:303-315)                     */
+#define CORDUM_PLAN_ALLOW_WITH_CONSTRAINTS 5 /* not routed (POLICY_ONLY), ALLOW_WITH_CONSTRAINTS: may dispatch (engine.go:299-302) */
+#define CORDUM_PLAN_MISSING_TOPIC 6      /* ROUTE_MISSING_TOPIC: not retryable, DLQ "dispatch_failed" (engine.go:393-406,470) */
+#define CORDUM_PLAN_NO_POOL_PREFERRED 7  /* ROUTE_NO_POOL_PREFERRED: ErrNoPoolMapping, DLQ "no_pool_mapping" (engine.go:403-406,462) */
+#define CORDUM_PLAN_NO_POOL_TOPIC 8      /* ROUTE_NO_POOL_TOPIC: as above (engine.go:403-406,462)                             */
+#define CORDUM_PLAN_NO_POOL_REQUIRES 9   /* ROUTE_NO_POOL_REQUIRES: as above (engine.go:403-406,462)                          */
+#define CORDUM_PLAN_NO_WORKERS 10        /* ROUTE_NO_WORKERS: ErrNoWorkers, RetryAfter(retryDelayNoWorkers) (engine.go:400-401) */
+#define CORDUM_PLAN_POOL_OVERLOADED 11   /* ROUTE_POOL_OVERLOADED: ErrPoolOverloaded, RetryAfter (engine.go:400-401)          */
+/* k = sched_decision (0..5) for jobs with route_status NOT_ATTEMPTED (in POLICY_ONLY mode every job), and
+ * k = 6 + route_status - CORDUM_ROUTE_MISSING_TOPIC (6..11) for the six route errors. */
+typedef struct cordum_plan {
+  uint32_t n_slots;        /* worker buckets = slots of the registry the batch was routed on (the batch's own, not the
+                              current one: cordum_subject resolves them against the same ids; 0 without a registry) */
+  uint32_t n_jobs;
+  const uint32_t* offsets; /* [n_slots + CORDUM_PLAN_OUTCOMES + 1]: bucket b holds jobs[offsets[b] .. offsets[b+1]);
+                              offsets[0] = 0, offsets[n_slots + CORDUM_PLAN_OUTCOMES] = n_jobs */
+  const uint32_t* jobs;    /* [n_jobs] original job indices (as in cordum_batch_results), grouped by bucket, ascending
+                              inside a bucket */
+} cordum_plan;
+/* Synchronous.  Valid once the batch's results are complete: after cordum_dispatch, or after cordum_batch_wait that
+ * follows an async, resident or tick dispatch (a device-encoded batch that fell back to the host encoder included).
+ * Before that, or for a batch never dispatched: CORDUM_E_STATE.  Both arrays are pinned memory owned by the batch, valid
+ * until its next encode, dispatch, plan or free.  Device scratch is O(n_jobs + buckets), grown on first need; when it
+ * does not fit the call is refused with CORDUM_E_CAPACITY and the engine stays usable.  Kernels are counted by
+ * cordum_launch_count. */
+int32_t cordum_batch_plan(cordum_batch* b, cordum_plan* out);
+
 /* Host-side materialisation of what the record indexes (pure functions of rule_idx /
  * reason_code / worker_slot; SURVEY.md A.5).  Each writes a NUL-terminated string
  * into buf (truncating to cap) and returns the full length. */

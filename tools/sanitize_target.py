@@ -1,6 +1,7 @@
 """Small end-to-end run of every kernel for compute-sanitizer (tools/sanitize.sh): policy_kernel, route_kernel (label
 picks, multi-chunk and unsorted pools), worker_chunk / worker_merge, the device encoder, heartbeat ingest, scheduler ticks,
-and the wide-mask path.  Checks the results against the oracle, so a sanitizer-clean run is also a correct one."""
+the wide-mask path and the dispatch plan kernels.  Checks the results against the oracle (the plan against a numpy
+grouping of the records), so a sanitizer-clean run is also a correct one."""
 import os
 import sys
 
@@ -22,6 +23,18 @@ def same(got, want, what):
     print("ok:", what, flush=True)
 
 
+def plan_same(b, rec, n_slots, what):
+    st = rec["route_status"].astype(np.int64)
+    routed = (st == wire.ROUTE_OK) | (st == wire.ROUTE_OK_PREFERRED)
+    key = np.where(routed, rec["worker_slot"].astype(np.int64),
+                   np.where(st == wire.ROUTE_NOT_ATTEMPTED, n_slots + rec["sched_decision"].astype(np.int64),
+                            n_slots + 6 + st - wire.ROUTE_MISSING_TOPIC))
+    offsets, jobs, ns = b.plan()
+    want = np.concatenate([[0], np.cumsum(np.bincount(key, minlength=n_slots + wire.PLAN_OUTCOMES))])
+    assert ns == n_slots and np.array_equal(offsets, want) and np.array_equal(jobs, np.argsort(key, kind="stable")), what
+    print("ok: plan,", what, flush=True)
+
+
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     light = len(sys.argv) > 2 and sys.argv[2] == "light"   # racecheck serialises everything: smaller pools, fewer phases
@@ -33,7 +46,9 @@ def main():
     o = oracle_lib.Oracle(cfg.policy, cfg.routing, cfg.workers)
     b = e.batch(n)
     for mode in (wire.MODE_POLICY_AND_ROUTE, wire.MODE_POLICY_ONLY, wire.MODE_ROUTE_ONLY):
-        same(b.encode(cfg.jobs).dispatch(mode), o.eval(cfg.jobs, mode), "c2 host-encode mode %d" % mode)
+        rec = b.encode(cfg.jobs).dispatch(mode)
+        same(rec, o.eval(cfg.jobs, mode), "c2 host-encode mode %d" % mode)
+        plan_same(b, rec, cfg.workers.n_workers, "c2 mode %d" % mode)   # 1,012 buckets: two radix passes
     same(b.encode_device(cfg.jobs).dispatch(), o.eval(cfg.jobs), "c2 device-encode")
     # heartbeat deltas + refresh
     rng = np.random.default_rng(3)
@@ -55,6 +70,7 @@ def main():
         jobs = [{"topic": "job.w.go", "labels": {"zone": "z%d" % (i % 4)}} for i in range(64)] + \
                [{"topic": "job.w.go", "labels": {"host": "m%05d" % (i % 97), "zone": "z%d" % (i % 4)}} for i in range(64)] + [{"topic": "job.w.go"}] * 8
         same(b.encode(jobs).dispatch(wire.MODE_ROUTE_ONLY), o2.eval(jobs, wire.MODE_ROUTE_ONLY), "pool of %d workers" % size)
+        plan_same(b, b.results(), size, "pool of %d workers" % size)
         o2.close()
     # wide masks
     sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -87,6 +103,7 @@ def main():
     b2.wait()                                  # routed by the flush, on the loads of the last tick
     o4.update_workers(np.arange(W, dtype=np.uint32), keep[3])
     same(b2.fetch(), o4.eval(cfg.jobs), "ticks")
+    plan_same(b2, b2.results(), W, "ticks")
     o4.close()
     o.close()
     print("sanitize target done", flush=True)
