@@ -167,6 +167,12 @@ struct cordum_batch {
   const cordum_envelopes* env = nullptr;   // the caller's envelopes, kept until the batch has been waited for (host fallback)
   DevBuf d_env, d_work;          // envelope arrays on the device; tid / ten / key / slot_of / hist / flag
   uint32_t* h_fallback = nullptr;   // pinned: 1 = the device encoder left something to the host
+  const uint32_t* d_slot_of = nullptr;   // device slot_of of records produced on the device (encoder work array or d_sub_idx)
+  // cordum_batch_subset, when this batch is the destination
+  bool is_subset = false;        // the records are a subset of another batch's: h_parent is valid
+  DevBuf d_sub_idx;              // [max_jobs] slot_of, then [max_jobs] parent index (allocated on first use)
+  DevBuf d_subset;               // scratch of the call (subset_batch), grown on first need
+  uint32_t* h_parent = nullptr;  // pinned [max_jobs]: source job index of each job
   uint32_t last_mode = 0;
   bool last_copy_out = false, timed = true;
   bool tick_pending = false;     // dispatched through cordum_tick_async: results are on the device once the tick streams have drained
@@ -649,6 +655,7 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->d_sel) cudaFree(b->d_sel);
   if (b->h_out) cudaFreeHost(b->h_out);
   if (b->h_plan) cudaFreeHost(b->h_plan);
+  if (b->h_parent) cudaFreeHost(b->h_parent);
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
   std::free(b->slot_of);
@@ -952,6 +959,7 @@ int host_encode_into(cordum_engine* e, cordum_batch* b, const cordum_envelopes* 
   b->resident = false;
   b->device_encoded = false;
   b->results_ready = false;
+  b->is_subset = false;
   uint64_t epoch_before = 0;
   int rc = CORDUM_OK;
   for (int attempt = 0; attempt < 3; ++attempt) {
@@ -1049,6 +1057,131 @@ int plan_batch(cordum_engine* e, cordum_batch* b, cordum_plan* out) {
             "was reloaded while the batch was in flight): encode and dispatch it again";
     return CORDUM_E_STALE;
   }
+  return CORDUM_OK;
+}
+
+// A new pinned + device pair of `bytes` each, for a subset's wide rows or selective list; both null when it does not fit.
+struct NewPair {
+  void *h = nullptr, *d = nullptr;
+  bool alloc(size_t bytes) {
+    if (cudaHostAlloc(&h, bytes, cudaHostAllocDefault) == cudaSuccess && cudaMalloc(&d, bytes) == cudaSuccess) return true;
+    cudaGetLastError();   // an allocation that does not fit is this call's problem, not a sticky engine failure
+    release();
+    return false;
+  }
+  void release() {
+    if (h) cudaFreeHost(h);
+    if (d) cudaFree(d);
+    h = d = nullptr;
+  }
+};
+
+// cordum_batch_subset once the arguments and both batches' states have been checked.  Scratch of dst (32-bit words):
+// jloc [n] | sloc [n] | eloc [2 n_sel] | jcnt, scnt [tiles] | ecnt, wcnt [sel tiles] | totals [4] | list [n_list].
+int subset_batch(cordum_engine* e, cordum_batch* src, uint32_t mask, const uint32_t* jobs, uint32_t n_list, cordum_batch* dst, uint32_t* n_out) {
+  SubsetParams P{};
+  const uint32_t n = src->n, n_sel = src->n_sel_jobs, T = CORDUM_SUBSET_TILE;
+  P.n = n;
+  P.n_sel = n_sel;
+  P.n_tiles = (uint32_t)(((uint64_t)n + T - 1) / T);
+  P.n_sel_tiles = (uint32_t)(((uint64_t)n_sel + T - 1) / T);
+  P.out = jobs ? nullptr : reinterpret_cast<const uint4*>(src->d_out);
+  P.mask = mask;
+  P.n_list = n_list;
+  JobRecords R;
+  device_records(src, R);
+  P.job = R.job; P.route = R.route; P.wide = R.wide; P.ww = src->wide_words;
+  P.sel_jobs = R.sel_jobs; P.sel_extra = R.sel_extra;
+  const size_t words = 2 * (size_t)n + 2 * (size_t)n_sel + 2 * (size_t)P.n_tiles + 2 * (size_t)P.n_sel_tiles + 4 + n_list;
+  const size_t idx_bytes = 2 * (size_t)dst->max_jobs * 4;
+  cudaError_t ae = dst->d_subset.reserve((words + words / 4) * 4);
+  if (ae == cudaSuccess) ae = dst->d_sub_idx.reserve(idx_bytes);
+  if (ae == cudaSuccess && !dst->h_parent) {
+    ae = cudaHostAlloc((void**)&dst->h_parent, (size_t)dst->max_jobs * 4, cudaHostAllocDefault);
+    if (ae != cudaSuccess) dst->h_parent = nullptr;   // allocated here: nothing of an earlier subset is lost
+  }
+  if (ae != cudaSuccess) {
+    cudaGetLastError();
+    g_err = "out of memory for the scratch of a subset of " + std::to_string(n) + " jobs";
+    return CORDUM_E_CAPACITY;
+  }
+  uint32_t* w = (uint32_t*)dst->d_subset.p;
+  P.jloc = w; P.sloc = w + n;
+  P.eloc = reinterpret_cast<uint2*>(w + 2 * (size_t)n);
+  P.jcnt = w + 2 * (size_t)n + 2 * (size_t)n_sel; P.scnt = P.jcnt + P.n_tiles;
+  P.ecnt = P.scnt + P.n_tiles; P.wcnt = P.ecnt + P.n_sel_tiles;
+  P.totals = P.wcnt + P.n_sel_tiles;
+  cudaStream_t s = dst->stream;
+  if (jobs) {
+    uint32_t* list = P.totals + 4;
+    if (n_list) CK(cudaMemcpyAsync(list, jobs, (size_t)n_list * 4, cudaMemcpyHostToDevice, s), "H2D subset list");
+    P.list = list;
+  }
+  // count: how many jobs, slots, selective entries and extra words the subset keeps
+  uint32_t totals[4] = {0, 0, 0, 0};
+  if (n) {
+    CK(launch_subset_count(P, s), "subset count kernels");
+    e->launches += subset_count_launches(P);
+    CK(cudaMemcpyAsync(totals, P.totals, sizeof totals, cudaMemcpyDeviceToHost, s), "D2H subset totals");
+  }
+  CK(cudaStreamSynchronize(s), "subset count");
+  const uint32_t m = totals[0];
+  if (totals[1] != m) { g_err = "the source batch's records do not index its jobs one to one"; return CORDUM_E_STATE; }
+  if (m > dst->max_jobs) {
+    g_err = "the subset has " + std::to_string(m) + " jobs, more than the destination batch holds (" + std::to_string(dst->max_jobs) + ")";
+    return CORDUM_E_CAPACITY;
+  }
+  // check capacity, then gather
+  P.m_sel = totals[2];
+  const uint64_t wide_need = (uint64_t)m * P.ww, sel_need = P.m_sel ? 2ull * P.m_sel + 1 + totals[3] : 0;
+  if (wide_need > dst->wide_cap || sel_need > dst->sel_cap) {
+    // Grown with the encoders' headroom (rows for m + m/4 jobs, at least 1,024; list words + words/4, at least 1,024).
+    // Both new pairs are allocated before either old one is released, so a refusal leaves dst as it was.
+    const uint64_t wide_want = wide_need > dst->wide_cap ? P.ww * std::min<uint64_t>(dst->max_jobs, std::max<uint64_t>(1024, (uint64_t)m + m / 4)) : 0;
+    const uint64_t sel_want = sel_need > dst->sel_cap ? std::max<uint64_t>(sel_need + sel_need / 4, 1024) : 0;
+    std::lock_guard<std::mutex> g(e->mu);
+    NewPair nw, ns;
+    if ((wide_want && !nw.alloc(wide_want * 8)) || (sel_want && !ns.alloc(sel_want * 4))) {
+      nw.release();
+      ns.release();
+      g_err = "out of memory for the wide-mask rows or the selective list of a subset of " + std::to_string(m) + " jobs";
+      return CORDUM_E_CAPACITY;
+    }
+    if (wide_want) {
+      if (dst->h_wide) cudaFreeHost(dst->h_wide);
+      if (dst->d_wide) cudaFree(dst->d_wide);
+      dst->h_wide = (uint64_t*)nw.h; dst->d_wide = (uint64_t*)nw.d; dst->wide_cap = wide_want;
+    }
+    if (sel_want) {
+      if (dst->h_sel) cudaFreeHost(dst->h_sel);
+      if (dst->d_sel) cudaFree(dst->d_sel);
+      dst->h_sel = (uint32_t*)ns.h; dst->d_sel = (uint32_t*)ns.d; dst->sel_cap = sel_want;
+    }
+    e->tables_gen++;   // captured tick graphs bake the batch's pointers in
+  }
+  P.djob = (JobRec*)dst->d_cols;
+  P.droute = (RouteRec*)(dst->d_cols + (size_t)m * sizeof(JobRec));
+  P.dwide = dst->d_wide;
+  P.dsel = dst->d_sel;
+  P.dslot_of = (uint32_t*)dst->d_sub_idx.p;
+  P.dparent = P.dslot_of + dst->max_jobs;
+  CK(launch_subset_gather(P, s), "subset gather kernel");
+  e->launches += subset_launches(P) - subset_count_launches(P);
+  if (m) CK(cudaMemcpyAsync(dst->h_parent, P.dparent, (size_t)m * 4, cudaMemcpyDeviceToHost, s), "D2H parent index");
+  CK(cudaStreamSynchronize(s), "subset gather");
+  dst->n = m;
+  dst->epoch = src->epoch;
+  dst->wide_words = P.ww;
+  dst->n_sel_jobs = P.m_sel;
+  dst->sel_words = (uint32_t)sel_need;
+  dst->d_slot_of = P.dslot_of;
+  dst->env = nullptr;
+  if (dst->h_fallback) *dst->h_fallback = 0;   // records produced here never go back to the host encoder
+  dst->encoded = dst->resident = dst->device_encoded = true;
+  dst->host_records_valid = false;
+  dst->results_ready = false;
+  dst->is_subset = true;
+  *n_out = m;
   return CORDUM_OK;
 }
 }  // namespace
@@ -1459,7 +1592,7 @@ int32_t cordum_encode_device(cordum_engine* e, cordum_batch* b, const cordum_env
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   const uint32_t n = env->n_jobs;
   b->n = n;
-  b->encoded = false; b->resident = false; b->device_encoded = false; b->results_ready = false;
+  b->encoded = false; b->resident = false; b->device_encoded = false; b->results_ready = false; b->is_subset = false;
   b->wide_words = 0;   // a batch the device encoder completes has none (wide tables raise the fallback flag)
   b->n_sel_jobs = b->sel_words = 0;   // nor a selective list (a selective pair raises it too)
   if (n == 0) { b->encoded = true; b->resident = true; b->device_encoded = true; b->host_records_valid = true; b->epoch = e->host->epoch(); return CORDUM_OK; }
@@ -1521,6 +1654,7 @@ int32_t cordum_encode_device(cordum_engine* e, cordum_batch* b, const cordum_env
   P.fallback = (uint32_t*)(w + 4 * arr + ((size_t)n_keys * 4 + 255) / 256 * 256);
   P.out_job = (JobRec*)b->d_cols;
   P.out_route = (RouteRec*)(b->d_cols + (size_t)n * sizeof(JobRec));
+  b->d_slot_of = P.slot_of;
   CK(launch_encode(P, n_keys, s), "encode kernels");
   e->launches += 3;
   CK(cudaMemcpyAsync(b->h_fallback, P.fallback, sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H fallback flag");
@@ -1539,8 +1673,7 @@ static int ensure_host_records(cordum_batch* b) {
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   host_records(b);
   CK(cudaMemcpy(b->h_cols, b->d_cols, slab_bytes(b->n), cudaMemcpyDeviceToHost), "D2H records");
-  const size_t arr = ((size_t)b->n * 4 + 255) / 256 * 256;
-  CK(cudaMemcpy(b->slot_of, (uint8_t*)b->d_work.p + 3 * arr, (size_t)b->n * 4, cudaMemcpyDeviceToHost), "D2H slot_of");
+  CK(cudaMemcpy(b->slot_of, b->d_slot_of, (size_t)b->n * 4, cudaMemcpyDeviceToHost), "D2H slot_of");
   b->host_records_valid = true;
   return CORDUM_OK;
 }
@@ -1594,6 +1727,42 @@ int32_t cordum_batch_plan(cordum_batch* b, cordum_plan* out) {
   if (!b->results_ready) { g_err = "the batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first"; return CORDUM_E_STATE; }
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   return plan_batch(e, b, out);
+}
+int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint32_t* jobs, uint32_t n_list, cordum_batch* dst, uint32_t* n_out) {
+  cordum::NvtxRange nvtx_("cordum:subset");
+  if (!src || !dst || !n_out) { g_err = "null argument"; return CORDUM_E_INVALID; }
+  if (src == dst) { g_err = "the subset must go to another batch than its source"; return CORDUM_E_INVALID; }
+  if (src->e != dst->e) { g_err = "the two batches belong to different engines"; return CORDUM_E_INVALID; }
+  if ((outcome_mask != 0) == (jobs != nullptr)) { g_err = "select by an outcome mask or by a job list, exactly one of the two"; return CORDUM_E_INVALID; }
+  if (outcome_mask >> CORDUM_PLAN_OUTCOMES) { g_err = "outcome mask names a bucket beyond CORDUM_PLAN_OUTCOMES"; return CORDUM_E_INVALID; }
+  for (uint32_t k = 0; jobs && k < n_list; ++k)
+    if (jobs[k] >= src->n || (k && jobs[k] <= jobs[k - 1])) {
+      g_err = "job list entry " + std::to_string(k) + " is out of range or not strictly ascending";
+      return CORDUM_E_INVALID;
+    }
+  cordum_engine* e = src->e;
+  if (e->failed) { g_err = "engine failed earlier: " + e->fail_msg; return CORDUM_E_CUDA; }
+  if (!jobs && !src->results_ready) {
+    g_err = "the source batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first";
+    return CORDUM_E_STATE;
+  }
+  if (jobs && (!src->encoded || !src->resident || src->pending || src->enc_inflight)) {
+    g_err = "the source batch's records are not complete on the device: wait for its encode or dispatch, or dispatch it once";
+    return CORDUM_E_STATE;
+  }
+  {
+    std::lock_guard<std::mutex> gh(e->host->mutex());
+    if (src->epoch != e->host->epoch()) { g_err = "tables were reloaded after the source batch was encoded: encode again"; return CORDUM_E_STALE; }
+  }
+  if (jobs && n_list > dst->max_jobs) { g_err = "the job list is longer than the destination batch holds"; return CORDUM_E_CAPACITY; }
+  if (dst->pending || dst->enc_inflight || dst->tick_pending) { int rc = wait(dst); if (rc) return rc; }
+  CK(cudaSetDevice(e->device), "cudaSetDevice");
+  return subset_batch(e, src, outcome_mask, jobs, n_list, dst, n_out);
+}
+const uint32_t* cordum_batch_parent_index(const cordum_batch* dst, uint32_t* n) {
+  const bool ok = dst && dst->is_subset;
+  if (n) *n = ok ? dst->n : 0;
+  return ok ? dst->h_parent : nullptr;
 }
 /* copies the decision records still on the device into the pinned result buffer (after a resident run) */
 int32_t cordum_batch_fetch(cordum_batch* b) {
@@ -1734,6 +1903,23 @@ int64_t cordum_test_canon(int32_t kind, const char* s, uint64_t n, char* buf, ui
   return (int64_t)o.size();
 }
 int32_t cordum_test_normalize_decision(const char* s, uint64_t n) { return cordum::normalize_decision_code(sv(s, n)); }
+/* a batch's side records as the kernels read them: which = 0 its selective list (32-bit words, tables.h JobRecords), 1 its
+ * wide-mask rows (64-bit words, [n][wide_words]).  Copies up to cap bytes into out; returns the full byte length, or -1 */
+int64_t cordum_test_batch_side(cordum_batch* b, int32_t which, void* out, uint64_t cap) {
+  if (!b || which < 0 || which > 1) return -1;
+  if ((b->pending || b->enc_inflight || b->tick_pending) && wait(b)) return -1;
+  const uint64_t bytes = which == 0 ? (uint64_t)b->sel_words * 4 : (uint64_t)b->n * b->wide_words * 8;
+  const void* dev = which == 0 ? (const void*)b->d_sel : (const void*)b->d_wide;
+  const void* host = which == 0 ? (const void*)b->h_sel : (const void*)b->h_wide;
+  const size_t take = (size_t)std::min<uint64_t>(bytes, cap);
+  if (take && b->resident) {   // what the last H2D put there, or what the device wrote
+    cordum_engine* e = b->e;
+    if (cudaSetDevice(e->device) != cudaSuccess || cudaMemcpy(out, dev, take, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+  } else if (take) {
+    std::memcpy(out, host, take);
+  }
+  return (int64_t)bytes;
+}
 int32_t cordum_test_parse_effective(const char* s, uint64_t n, uint32_t* n_allowed, uint32_t* n_denied) {
   cordum::EffSafety cfg;
   bool ok = cordum::parse_effective_safety(sv(s, n), cfg);

@@ -59,6 +59,45 @@ uint32_t plan_passes(uint32_t n_buckets);
 cudaError_t launch_plan(const PlanParams& P, cudaStream_t s);
 inline uint32_t plan_launches(const PlanParams& P) { return P.n ? 3u * plan_passes(P.n_buckets) + 1u : 0u; }
 
+// ---- batch subsets (subset.cu): a new encoded batch from a chosen subset of an encoded one (cordum_batch_subset)
+#define CORDUM_SUBSET_TILE 2048u   // items (jobs, sorted slots or selective-list entries) per CTA
+#define CORDUM_SUBSET_NONE 0xFFFFFFFFu
+struct SubsetParams {
+  // source batch (device)
+  uint32_t n;                      // jobs
+  const uint4* out;                // selection by outcome: the decision records (caller order); null for a list
+  uint32_t mask;                   // outcome buckets selected (bit k = CORDUM_PLAN_* k)
+  const uint32_t* list;            // selection by list: ascending job indices; null for an outcome mask
+  uint32_t n_list;
+  const JobRec* job;
+  const RouteRec* route;
+  const uint64_t* wide;            // [n][ww] or null
+  uint32_t ww;
+  const uint2* sel_jobs;           // the selective list (tables.h JobRecords) or null
+  const uint32_t* sel_extra;
+  uint32_t n_sel;
+  uint32_t n_tiles, n_sel_tiles;   // tiles of n jobs / slots, and of n_sel entries
+  // scratch (device)
+  uint32_t* jloc;                  // [n] per job: rank among the selected jobs of its tile, or NONE
+  uint32_t* sloc;                  // [n] per sorted slot: rank among the kept slots of its tile, or NONE
+  uint2* eloc;                     // [n_sel] per entry: {rank among the tile's kept entries or NONE, its extra words' offset}
+  uint32_t *jcnt, *scnt, *ecnt, *wcnt;   // per tile counts; exclusive prefixes over the tiles after the scan
+  uint32_t* totals;                // [4]: selected jobs, kept slots, kept entries, their extra words
+  // destination batch (device)
+  JobRec* djob;
+  RouteRec* droute;
+  uint64_t* dwide;                 // [m][ww]
+  uint32_t* dsel;                  // [2 m_sel] {slot, x}, then the extra words
+  uint32_t m_sel;
+  uint32_t* dslot_of;              // [m]
+  uint32_t* dparent;               // [m] source job index of each new job
+};
+// mark -> keep -> scan, then (after the host has read totals and sized the destination) gather
+cudaError_t launch_subset_count(const SubsetParams& P, cudaStream_t s);
+cudaError_t launch_subset_gather(const SubsetParams& P, cudaStream_t s);
+inline uint32_t subset_count_launches(const SubsetParams& P) { return P.n ? 3u : 0u; }
+inline uint32_t subset_launches(const SubsetParams& P) { return P.n ? 4u : 0u; }
+
 // ---- device-side encoder (encode.cu)
 struct EncodeParams {
   uint32_t n_jobs;

@@ -139,6 +139,29 @@ class Batch:
         for b in np.flatnonzero(np.diff(offsets)):
             yield int(b), jobs[offsets[b]:offsets[b + 1]]
 
+    def subset(self, dst: "Batch", outcomes: int = None, jobs=None) -> int:
+        """Make `dst` the encoded batch of a subset of this one (cordum_batch_subset), on the device: the jobs whose plan
+        outcome bucket k has bit k set in `outcomes` (e.g. wire.SUBSET_RETRYABLE), or the strictly ascending job indices
+        `jobs`.  Returns dst's job count; dst.parent_index() maps its jobs back to this batch's."""
+        m = C.c_uint32()
+        if jobs is None:
+            self.eng._ck(self.L.cordum_batch_subset(self.h, outcomes or 0, None, 0, dst.h, C.byref(m)))
+        else:
+            lst = np.ascontiguousarray(jobs, dtype=np.uint32)
+            buf = lst if len(lst) else np.zeros(1, np.uint32)   # the empty list is a list: a non-null pointer
+            self.eng._ck(self.L.cordum_batch_subset(self.h, outcomes or 0, C.c_void_p(buf.ctypes.data), len(lst), dst.h, C.byref(m)))
+        dst._env = None   # dst holds no envelopes: MCP reasons quote the canonical spelling
+        return m.value
+
+    def parent_index(self) -> np.ndarray:
+        """This batch's job i -> the source batch's job index, when its records came from Batch.subset (else empty).  A
+        view of library memory, valid until this batch's next encode, subset or free."""
+        n = C.c_uint32()
+        ptr = self.L.cordum_batch_parent_index(self.h, C.byref(n))
+        if not ptr or not n.value:
+            return np.zeros(0, np.uint32)
+        return np.frombuffer((C.c_uint32 * n.value).from_address(ptr), dtype=np.uint32, count=n.value)
+
     def _text(self, fn, job: int, *extra) -> str:
         buf = C.create_string_buffer(4096)
         n = fn(self.eng.h, self.h, job, *extra, buf, len(buf))

@@ -152,6 +152,9 @@ FLAG_NO_TIMING = 0x200
 # dispatch plan: bucket n_slots + k holds the jobs of outcome k (include/cordum_b200.h CORDUM_PLAN_*)
 PLAN_OUTCOMES = 12
 PLAN_OUTCOME_NAMES = DEC_NAMES + ["MISSING_TOPIC", "NO_POOL_PREFERRED", "NO_POOL_TOPIC", "NO_POOL_REQUIRES", "NO_WORKERS", "POOL_OVERLOADED"]
+# batch subsets: outcome buckets the scheduler retries (include/cordum_b200.h CORDUM_SUBSET_RETRYABLE)
+PLAN_THROTTLE, PLAN_NO_WORKERS, PLAN_POOL_OVERLOADED = 4, 10, 11
+SUBSET_RETRYABLE = (1 << PLAN_THROTTLE) | (1 << PLAN_NO_WORKERS) | (1 << PLAN_POOL_OVERLOADED)
 REASON_NONE, REASON_RULE, REASON_MISSING_TOPIC, REASON_UNSUPPORTED_TOPIC, REASON_TENANT_MCP = 0, 1, 2, 3, 4
 REASON_EFF_DENIED_TOPIC, REASON_EFF_NOT_ALLOWED_TOPIC, REASON_EFF_MCP, REASON_APPROVAL_GRANTED = 12, 13, 14, 22
 

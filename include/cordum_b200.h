@@ -381,6 +381,38 @@ typedef struct cordum_plan {
  * cordum_launch_count. */
 int32_t cordum_batch_plan(cordum_batch* b, cordum_plan* out);
 
+/* ---- batch subsets: requeue part of an encoded batch without encoding it again.  A job the scheduler retries
+ * (THROTTLE, NO_WORKERS, POOL_OVERLOADED: RetryAfter, engine.go:303-315, 393-402; or a routed job whose publish failed,
+ * engine.go:420-441) goes through checkSafetyDecision and PickSubject again on redelivery.  cordum_batch_subset builds
+ * that retry batch on the device from the source's encoded records, which stay valid as long as its table epoch
+ * (heartbeat deltas keep the epoch), so no strings are resolved and nothing crosses PCIe but the selection.
+ *
+ * Selection, exactly one of the two:
+ *   outcome_mask != 0, jobs == NULL: every src job whose plan outcome bucket k (CORDUM_PLAN_*, 0..11) has bit k set.
+ *     Needs src's results complete, as cordum_batch_plan does (after cordum_dispatch, or cordum_batch_wait after an
+ *     async, resident or tick dispatch); else CORDUM_E_STATE.
+ *   outcome_mask == 0, jobs != NULL: n_list strictly ascending src job indices (e.g. one worker bucket of a plan).
+ *     Needs src's records complete on the device: a device encode that has been waited for without falling back, or a
+ *     batch dispatched at least once and not in flight; else CORDUM_E_STATE (a host-encoded batch never dispatched).
+ * Result: dst becomes an encoded batch of m = *n_out jobs (0 allowed), resident on the device: src's sorted records
+ * restricted to the selection in the same order, JobRec.orig renumbered to the job's rank among the selected src indices,
+ * wide rows and the selective list carried over in the host encoder's layout, src's table epoch.  dst keeps no pointer to
+ * src or to its envelopes (src may be re-encoded or freed) and never falls back to the host encoder.  Every dispatch form
+ * (blocking, async, resident, cordum_tick_async) runs dst without copying records in; cordum_batch_plan, cordum_reason*
+ * (MCP values in their canonical spelling), cordum_subject and cordum_batch_records work on it.
+ * Synchronous: the jobs are counted on the device, the capacity checked, then the records gathered (4 kernel launches,
+ * counted by cordum_launch_count; 0 for an empty src).
+ * Refusals: CORDUM_E_INVALID for src == dst, batches of different engines, both selectors or neither, mask bits >= 12,
+ * or a list that is unsorted, repeats an index or is out of range.  CORDUM_E_STALE when the tables were reloaded after
+ * src was encoded (policy, routing, workers, or a new dictionary generation).  CORDUM_E_CAPACITY when m exceeds dst's
+ * max_jobs (checked before any device work for a list) or the scratch does not fit; dst is then left as it was. */
+#define CORDUM_SUBSET_RETRYABLE ((1u << CORDUM_PLAN_THROTTLE) | (1u << CORDUM_PLAN_NO_WORKERS) | (1u << CORDUM_PLAN_POOL_OVERLOADED))
+int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint32_t* jobs, uint32_t n_list,
+                            cordum_batch* dst, uint32_t* n_out);
+/* dst job i -> its src job index, ascending; n = dst's job count.  Pinned memory owned by dst, valid until dst's next
+ * encode, subset or free.  NULL (n = 0) when dst's records did not come from cordum_batch_subset. */
+const uint32_t* cordum_batch_parent_index(const cordum_batch* dst, uint32_t* n);
+
 /* Host-side materialisation of what the record indexes (pure functions of rule_idx /
  * reason_code / worker_slot; SURVEY.md A.5).  Each writes a NUL-terminated string
  * into buf (truncating to cap) and returns the full length. */

@@ -1,7 +1,8 @@
 """Small end-to-end run of every kernel for compute-sanitizer (tools/sanitize.sh): policy_kernel, route_kernel (label
 picks, multi-chunk and unsorted pools), worker_chunk / worker_merge, the device encoder, heartbeat ingest, scheduler ticks,
-the wide-mask path and the dispatch plan kernels.  Checks the results against the oracle (the plan against a numpy
-grouping of the records), so a sanitizer-clean run is also a correct one."""
+the wide-mask path, the dispatch plan kernels and the batch subset kernels.  Checks the results against the oracle (the
+plan against a numpy grouping of the records, a subset against its source's records), so a sanitizer-clean run is also a
+correct one."""
 import os
 import sys
 
@@ -35,6 +36,19 @@ def plan_same(b, rec, n_slots, what):
     print("ok: plan,", what, flush=True)
 
 
+def subset_same(b, dst, rec, what):
+    """A subset by outcome and one by list (across a tile edge), dispatched: each job decides as its source job did."""
+    st = rec["route_status"]
+    for kw in ({"outcomes": (1 << wire.PLAN_OUTCOMES) - 1}, {"jobs": np.arange(1, len(rec), 3)}):
+        m = b.subset(dst, **kw)
+        parent = dst.parent_index().copy()
+        if "jobs" in kw:
+            assert np.array_equal(parent, kw["jobs"]), what
+        else:
+            assert np.array_equal(parent, np.flatnonzero((st != wire.ROUTE_OK) & (st != wire.ROUTE_OK_PREFERRED))), what
+        same(dst.dispatch().copy()[:m], rec[parent], "subset (%s), %s" % (sorted(kw)[0], what))
+
+
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     light = len(sys.argv) > 2 and sys.argv[2] == "light"   # racecheck serialises everything: smaller pools, fewer phases
@@ -60,6 +74,8 @@ def main():
     e.update_workers(slots, loads)
     o.update_workers(slots, loads)
     same(b.encode(cfg.jobs).dispatch(), o.eval(cfg.jobs), "after heartbeat deltas")
+    dst = e.batch(n)
+    subset_same(b, dst, b.results().copy(), "c2")
     # one big pool: multi-chunk merge (1300) and beyond the sort buffer (9000)
     for size in ((1300,) if light else (1300, 9000)):
         routing = {"topics": {"job.w.go": ["big"]}, "pools": {"big": {}}}
@@ -83,7 +99,18 @@ def main():
     o3 = oracle_lib.Oracle(policy, routing, workers)
     bw = e.batch(len(jobs))
     same(bw.encode(jobs).dispatch(), o3.eval(jobs), "wide masks")
+    subset_same(bw, e.batch(len(jobs)), bw.results().copy(), "wide masks")
     o3.close()
+    # selective placement pairs: the subset re-packs the selective list and its extra words
+    import test_selective_differential as tsd
+
+    policy, routing, workers = tsd.pins_registry()
+    jobs = tsd.pins_jobs(workers)[: 300 if light else None]
+    e.load_policy(policy, "pins")
+    e.load_routing(routing)
+    e.load_workers(workers)
+    bs = e.batch(len(jobs))
+    subset_same(bs, e.batch(len(jobs)), bs.encode(jobs).dispatch().copy(), "selective pairs")
     # scheduler ticks on the c2 tables
     e.load_policy(cfg.policy, "san2")
     e.load_routing(cfg.routing)
