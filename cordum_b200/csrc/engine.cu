@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -183,6 +184,9 @@ struct cordum_batch {
   DevBuf d_plan;                 // cordum_batch_plan scratch (plan_batch), grown on first need
   uint32_t* h_plan = nullptr;    // pinned: the plan's offsets, the record-check flag, then its jobs
   size_t h_plan_cap = 0;         // 32-bit words
+  DevBuf d_counts;               // cordum_batch_topic_counts scratch (count_batch), grown on first need
+  uint32_t* h_counts = nullptr;  // pinned: the copied topic rows, then the output (counts | label offsets | label bytes)
+  size_t h_counts_cap = 0;       // 32-bit words
   uint2* d_route = nullptr;           // [0].x = count, [2..] = compacted list of dispatchable jobs {slot, head}
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, ev2 = nullptr, ev3 = nullptr;
@@ -655,6 +659,7 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->d_sel) cudaFree(b->d_sel);
   if (b->h_out) cudaFreeHost(b->h_out);
   if (b->h_plan) cudaFreeHost(b->h_plan);
+  if (b->h_counts) cudaFreeHost(b->h_counts);
   if (b->h_parent) cudaFreeHost(b->h_parent);
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
@@ -1057,6 +1062,112 @@ int plan_batch(cordum_engine* e, cordum_batch* b, cordum_plan* out) {
             "was reloaded while the batch was in flight): encode and dispatch it again";
     return CORDUM_E_STALE;
   }
+  return CORDUM_OK;
+}
+
+// The batch's pinned topic-count buffer, grown to at least `words` 32-bit words; false (buffer released) when it does not fit.
+bool counts_host_reserve(cordum_batch* b, size_t words) {
+  if (words <= b->h_counts_cap) return true;
+  if (b->h_counts) cudaFreeHost(b->h_counts);
+  b->h_counts = nullptr; b->h_counts_cap = 0;
+  const size_t want = std::max<size_t>(words + words / 4, 64);
+  if (cudaHostAlloc((void**)&b->h_counts, want * 4, cudaHostAllocDefault) != cudaSuccess) {
+    cudaGetLastError();   // an allocation that does not fit is this call's problem, not a sticky engine failure
+    b->h_counts = nullptr;
+    return false;
+  }
+  b->h_counts_cap = want;
+  return true;
+}
+
+// cordum_batch_topic_counts on a batch whose records are complete in d_out.  Device scratch (32-bit words): table
+// [n_topics][13] | head [2] | rows [n_topics][14].  Pinned: the copied non-zero rows; once they are merged by label, the
+// output: counts [n_rows][13] | label offsets [n_rows + 1] | label bytes.
+int count_batch(cordum_engine* e, cordum_batch* b, cordum_topic_counts* out) {
+  constexpr uint32_t C = CORDUM_COUNT_COLUMNS;
+  CountParams P{};
+  JobRecords R;
+  device_records(b, R);
+  P.job = R.job;
+  P.out = reinterpret_cast<const uint4*>(b->d_out);
+  P.n = b->n;
+  P.n_slots = b->wtext ? (uint32_t)b->wtext->size() : 0u;   // the registry the batch was routed on
+  {
+    std::lock_guard<std::mutex> g(e->host->mutex());        // a generation's topic store grows under this lock
+    P.n_topics = b->ttext ? (uint32_t)b->ttext->size() : 0u;
+  }
+  const size_t nt = P.n_topics, dev_words = P.n ? nt * C + 2 + nt * (C + 1) : 0;
+  const cudaError_t de = dev_words * 4 > b->d_counts.cap ? b->d_counts.reserve(dev_words * 5) : cudaSuccess;   // + 1/4
+  if (de != cudaSuccess || !counts_host_reserve(b, 2)) {
+    cudaGetLastError();
+    g_err = "out of memory for the topic counts of " + std::to_string(P.n) + " jobs over " + std::to_string(nt) + " topic ids";
+    return CORDUM_E_CAPACITY;
+  }
+  out->n_jobs = P.n;
+  if (P.n == 0) {
+    b->h_counts[0] = 0;
+    out->n_rows = 0;
+    out->counts = out->label_off = b->h_counts;
+    out->label_bytes = reinterpret_cast<const uint8_t*>(b->h_counts + 1);
+    return CORDUM_OK;
+  }
+  uint32_t* w = (uint32_t*)b->d_counts.p;
+  P.table = w;
+  P.head = w + nt * C;
+  P.rows = P.head + 2;
+  cudaStream_t s = b->stream;
+  CK(launch_counts(P, s), "topic count kernels");
+  e->launches += counts_launches(P);
+  CK(cudaMemcpyAsync(b->h_counts, P.head, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H topic count head");
+  CK(cudaStreamSynchronize(s), "topic counts");
+  if (b->h_counts[1]) {
+    g_err = "a decision record of this batch names a worker slot outside the registry it was dispatched against (the registry "
+            "was reloaded while the batch was in flight): encode and dispatch it again";
+    return CORDUM_E_STALE;
+  }
+  const uint32_t m = b->h_counts[0];
+  if (!counts_host_reserve(b, (size_t)m * (C + 1))) {
+    g_err = "out of memory for the " + std::to_string(m) + " topic rows of a batch";
+    return CORDUM_E_CAPACITY;
+  }
+  if (m) CK(cudaMemcpyAsync(b->h_counts, P.rows, (size_t)m * (C + 1) * 4, cudaMemcpyDeviceToHost, s), "D2H topic rows");
+  CK(cudaStreamSynchronize(s), "topic rows");
+  // merge by label, TrimSpace(raw topic) in the batch's dictionary generation, and order the rows by label bytes
+  // (std::string compares as unsigned char)
+  struct Row { std::string label; uint32_t cnt[C]; };
+  std::vector<Row> rows(m);
+  {
+    std::lock_guard<std::mutex> g(e->host->mutex());
+    for (uint32_t i = 0; i < m; ++i) {
+      const uint32_t* r = b->h_counts + (size_t)i * (C + 1);
+      rows[i].label = std::string(cordum::trim_space((*b->ttext)[r[0]]));   // r[0] < n_topics: the kernel checked it
+      std::memcpy(rows[i].cnt, r + 1, sizeof rows[i].cnt);
+    }
+  }
+  std::sort(rows.begin(), rows.end(), [](const Row& x, const Row& y) { return x.label < y.label; });
+  std::vector<uint32_t> cnt, off{0};
+  std::string bytes;
+  for (uint32_t i = 0; i < m; ++i) {
+    if (i == 0 || rows[i].label != rows[i - 1].label) {
+      cnt.resize(cnt.size() + C, 0);
+      bytes += rows[i].label;
+      off.push_back((uint32_t)bytes.size());
+    }
+    for (uint32_t c = 0; c < C; ++c) cnt[cnt.size() - C + c] += rows[i].cnt[c];
+  }
+  const uint32_t n_rows = (uint32_t)off.size() - 1;
+  if (!counts_host_reserve(b, cnt.size() + off.size() + (bytes.size() + 3) / 4)) {
+    g_err = "out of memory for the topic counts of " + std::to_string(n_rows) + " labels";
+    return CORDUM_E_CAPACITY;
+  }
+  uint32_t* h = b->h_counts;
+  std::memcpy(h, cnt.data(), cnt.size() * 4);
+  std::memcpy(h + cnt.size(), off.data(), off.size() * 4);
+  std::memcpy(h + cnt.size() + off.size(), bytes.data(), bytes.size());
+  out->n_rows = n_rows;
+  out->counts = h;
+  out->label_off = h + cnt.size();
+  out->label_bytes = reinterpret_cast<const uint8_t*>(h + cnt.size() + off.size());
   return CORDUM_OK;
 }
 
@@ -1727,6 +1838,15 @@ int32_t cordum_batch_plan(cordum_batch* b, cordum_plan* out) {
   if (!b->results_ready) { g_err = "the batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first"; return CORDUM_E_STATE; }
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   return plan_batch(e, b, out);
+}
+int32_t cordum_batch_topic_counts(cordum_batch* b, cordum_topic_counts* out) {
+  cordum::NvtxRange nvtx_("cordum:topic_counts");
+  if (!b || !out) { g_err = "null argument"; return CORDUM_E_INVALID; }
+  cordum_engine* e = b->e;
+  if (e->failed) { g_err = "engine failed earlier: " + e->fail_msg; return CORDUM_E_CUDA; }
+  if (!b->results_ready) { g_err = "the batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first"; return CORDUM_E_STATE; }
+  CK(cudaSetDevice(e->device), "cudaSetDevice");
+  return count_batch(e, b, out);
 }
 int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint32_t* jobs, uint32_t n_list, cordum_batch* dst, uint32_t* n_out) {
   cordum::NvtxRange nvtx_("cordum:subset");

@@ -38,6 +38,18 @@ inline uint32_t route_launches(const KParams& P) { return P.n_jobs ? 1u + (P.t.n
 
 // ---- batch dispatch plan (plan.cu): the jobs of a batch grouped by bucket key (include/cordum_b200.h cordum_plan)
 #define CORDUM_PLAN_TILE 2048u   // jobs per CTA of the count / scatter kernels
+#define CORDUM_PLAN_NONE 0xFFFFFFFFu
+// Outcome of a decision record, head = its first word (cordum_decision bytes 0..3), as the plan (plan.cu), the subsets
+// (subset.cu) and the topic counts (counts.cu) classify it: the outcome bucket k (CORDUM_PLAN_*, 0..11) of a job that was
+// not routed, CORDUM_COUNT_ROUTED for a routed one (its worker slot names the plan's bucket), CORDUM_PLAN_NONE for a
+// record that fits no bucket.
+__device__ __forceinline__ uint32_t plan_outcome(uint32_t head) {
+  const uint32_t sched = (head >> 8) & 0xFFu, status = head >> 24;   // sched_decision, route_status
+  if (status == CORDUM_ROUTE_OK || status == CORDUM_ROUTE_OK_PREFERRED) return CORDUM_COUNT_ROUTED;
+  if (status == CORDUM_ROUTE_NOT_ATTEMPTED) return sched <= CORDUM_DEC_ALLOW_WITH_CONSTRAINTS ? sched : CORDUM_PLAN_NONE;
+  if (status <= CORDUM_ROUTE_POOL_OVERLOADED) return CORDUM_PLAN_MISSING_TOPIC + (status - CORDUM_ROUTE_MISSING_TOPIC);
+  return CORDUM_PLAN_NONE;
+}
 struct PlanPass {                // one 8-bit radix pass
   const uint4* recs;             // pass 0: the decision records (keys are derived from them); later passes: null
   const uint32_t *keys_in, *vals_in;
@@ -97,6 +109,21 @@ cudaError_t launch_subset_count(const SubsetParams& P, cudaStream_t s);
 cudaError_t launch_subset_gather(const SubsetParams& P, cudaStream_t s);
 inline uint32_t subset_count_launches(const SubsetParams& P) { return P.n ? 3u : 0u; }
 inline uint32_t subset_launches(const SubsetParams& P) { return P.n ? 4u : 0u; }
+
+// ---- per-topic outcome counts (counts.cu): a dispatched batch's jobs counted per (topic id, outcome column)
+#define CORDUM_COUNT_TILE 2048u     // sorted records per CTA of the count kernel
+#define CORDUM_COUNT_WINDOW 64u     // topic ids, from the tile's first one on, that a CTA adds up in shared memory
+struct CountParams {
+  const JobRec* job;                // device: the batch's sorted records (topic, orig)
+  const uint4* out;                 // device: its decision records, caller order
+  uint32_t n, n_slots, n_topics;    // jobs; slots of the registry it was routed on; topic ids of its dictionary generation
+  uint32_t* table;                  // [n_topics][CORDUM_COUNT_COLUMNS]
+  uint32_t* head;                   // [2]: non-zero rows, record-check flag (raised when a record fits no bucket)
+  uint32_t* rows;                   // [n_topics][1 + CORDUM_COUNT_COLUMNS]: {topic id, counts} of the non-zero rows, any order
+};
+// zeroes table and head, counts, compacts the non-zero rows (rows[0 .. head[0]))
+cudaError_t launch_counts(const CountParams& P, cudaStream_t s);
+inline uint32_t counts_launches(const CountParams& P) { return P.n ? 2u : 0u; }
 
 // ---- device-side encoder (encode.cu)
 struct EncodeParams {

@@ -27,14 +27,12 @@ constexpr uint32_t kNone = 0xFFFFFFFFu;   // a lane with no job in this round
 
 // Bucket key of one decision record (the header's cordum_plan); a record that fits no bucket raises *bad and counts as 0.
 __device__ __forceinline__ uint32_t plan_key(uint4 rec, uint32_t n_slots, uint32_t* bad) {
-  const uint32_t sched = (rec.x >> 8) & 0xFFu, status = rec.x >> 24, slot = rec.w;   // cordum_decision bytes 1, 3; worker_slot
+  const uint32_t o = plan_outcome(rec.x), slot = rec.w;   // worker_slot
   uint32_t k = kNone;
-  if (status == CORDUM_ROUTE_OK || status == CORDUM_ROUTE_OK_PREFERRED) {
+  if (o == CORDUM_COUNT_ROUTED) {
     if (slot < n_slots) k = slot;
-  } else if (status == CORDUM_ROUTE_NOT_ATTEMPTED) {
-    if (sched <= CORDUM_DEC_ALLOW_WITH_CONSTRAINTS) k = n_slots + sched;
-  } else if (status <= CORDUM_ROUTE_POOL_OVERLOADED) {
-    k = n_slots + CORDUM_PLAN_MISSING_TOPIC + (status - CORDUM_ROUTE_MISSING_TOPIC);
+  } else if (o != CORDUM_PLAN_NONE) {
+    k = n_slots + o;
   }
   if (k == kNone) {   // e.g. a worker slot beyond the registry the batch was routed on: the host refuses the plan
     atomicOr(bad, 1u);

@@ -63,11 +63,8 @@ __device__ __forceinline__ void tile_scan(const uint32_t (&v)[kItems], uint32_t 
 
 // Outcome bucket of a decision record (include/cordum_b200.h CORDUM_PLAN_*), or NONE for a routed job.
 __device__ __forceinline__ uint32_t outcome_of(uint4 rec) {
-  const uint32_t sched = (rec.x >> 8) & 0xFFu, status = rec.x >> 24;   // cordum_decision bytes 1, 3
-  if (status == CORDUM_ROUTE_NOT_ATTEMPTED) return sched <= CORDUM_DEC_ALLOW_WITH_CONSTRAINTS ? sched : kNone;
-  if (status >= CORDUM_ROUTE_MISSING_TOPIC && status <= CORDUM_ROUTE_POOL_OVERLOADED)
-    return CORDUM_PLAN_MISSING_TOPIC + (status - CORDUM_ROUTE_MISSING_TOPIC);
-  return kNone;
+  const uint32_t k = plan_outcome(rec.x);
+  return k < CORDUM_PLAN_OUTCOMES ? k : kNone;
 }
 
 __global__ void __launch_bounds__(kThreads) subset_mark_kernel(SubsetParams P) {

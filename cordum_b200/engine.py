@@ -139,6 +139,23 @@ class Batch:
         for b in np.flatnonzero(np.diff(offsets)):
             yield int(b), jobs[offsets[b]:offsets[b + 1]]
 
+    def topic_counts(self):
+        """(labels, counts) of the last completed dispatch (cordum_batch_topic_counts): labels = the distinct
+        TrimSpace(topic) of its jobs as bytes, ascending; counts = uint32 [len(labels), wire.COUNT_COLUMNS], column k <
+        wire.PLAN_OUTCOMES the jobs of plan outcome k, column wire.COUNT_ROUTED the routed jobs.  The counts are a view of
+        library memory, valid until this batch's next encode, dispatch, topic_counts or free."""
+        t = wire.CordumTopicCounts()
+        self.eng._ck(self.L.cordum_batch_topic_counts(self.h, C.byref(t)))
+        n = t.n_rows
+        if not n:
+            return [], np.zeros((0, wire.COUNT_COLUMNS), np.uint32)
+        off = np.frombuffer((C.c_uint32 * (n + 1)).from_address(t.label_off), dtype=np.uint32, count=n + 1)
+        raw = C.string_at(t.label_bytes, int(off[n])) if off[n] else b""
+        labels = [raw[off[r]:off[r + 1]] for r in range(n)]
+        counts = np.frombuffer((C.c_uint32 * (n * wire.COUNT_COLUMNS)).from_address(t.counts), dtype=np.uint32,
+                               count=n * wire.COUNT_COLUMNS).reshape(n, wire.COUNT_COLUMNS)
+        return labels, counts
+
     def subset(self, dst: "Batch", outcomes: int = None, jobs=None) -> int:
         """Make `dst` the encoded batch of a subset of this one (cordum_batch_subset), on the device: the jobs whose plan
         outcome bucket k has bit k set in `outcomes` (e.g. wire.SUBSET_RETRYABLE), or the strictly ascending job indices

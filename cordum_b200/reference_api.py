@@ -12,6 +12,7 @@ tests read like the reference's own:
   LeastLoadedStrategy.{pick_subject,update_routing,current_routing}                strategy_least_loaded.go:21-136
   MemoryRegistry.{update_heartbeat,snapshot} scheduler.MemoryRegistry              registry_memory.go:11-84
   Scheduler.process_jobs                     Engine.processJob's decision switch   engine.go:294-347,393
+  topic_metrics(labels, counts)              the four topic-labelled counters      metrics/metrics.go:48-70
 
 Requests are plain dicts shaped like the CAP v2 messages (SURVEY App. B).  Every decision and
 every routed subject comes from the GPU (cordum_dispatch); this module only maps fields,
@@ -367,3 +368,43 @@ class Scheduler:
                         "rule_id": self.engine.rule_id(int(rec["rule_idx"])) if rec["rule_idx"] >= 0 else "",
                         "approval_required": bool(rec["flags"] & wire.F_APPROVAL_REQUIRED), "subject": subject, "error": err})
         return out
+
+
+JOB_STATUS_FAILED = "JOB_STATUS_FAILED"   # pb.JobStatus_JOB_STATUS_FAILED.String()
+
+
+def topic_metrics(labels: list[bytes], counts: np.ndarray) -> dict:
+    """What handleJobRequest / processJob add to the four counter vectors of metrics.Prom (metrics/metrics.go:48-70) for
+    the jobs of one table of Batch.topic_counts(): {"jobs_received_total": {topic: n}, "safety_denied_total": {topic: n},
+    "jobs_completed_total": {(topic, status): n}, "jobs_dispatched_total": {topic: n}}, topics as the label bytes, zero
+    increments left out (a counter child exists once it has been incremented).
+
+    - The "" row is an invalid request (engine.go:209-218): the whole row goes to completed{"", FAILED} and nothing else.
+    - received = the row's total (engine.go:239).
+    - safety_denied = DENY + UNSPECIFIED (engine.go:333, :344).
+    - completed{FAILED} = MISSING_TOPIC + the three NO_POOL columns: PickSubject errors that are not retryable
+      (engine.go:404).
+    - dispatched = the routed column (engine.go:435).  The reference increments it only after bus.Publish succeeded, so a
+      caller subtracts the jobs of the worker buckets whose publish failed (those are retried, engine.go:426-433).
+    - THROTTLE, NO_WORKERS, POOL_OVERLOADED (retried) and REQUIRE_HUMAN (awaits approval) increment nothing; ALLOW and
+      ALLOW_WITH_CONSTRAINTS without routing (POLICY_ONLY) neither.
+    The store gates before engine.go:239 (job lock, terminal or dispatched state) are the caller's: they keep a job from
+    reaching any of these lines."""
+    counts = np.asarray(counts, dtype=np.int64).reshape(len(labels), wire.COUNT_COLUMNS)
+    received, denied, completed, dispatched = {}, {}, {}, {}
+
+    def add(d, key, v):
+        if v:
+            d[key] = d.get(key, 0) + int(v)
+
+    for label, row in zip(labels, counts):
+        label = bytes(label)
+        if label == b"":
+            add(completed, (label, JOB_STATUS_FAILED), row.sum())
+            continue
+        add(received, label, row.sum())
+        add(denied, label, row[wire.DEC_DENY] + row[wire.DEC_UNSPECIFIED])
+        add(completed, (label, JOB_STATUS_FAILED), row[6:wire.PLAN_NO_WORKERS].sum())   # MISSING_TOPIC, NO_POOL_*
+        add(dispatched, label, row[wire.COUNT_ROUTED])
+    return {"jobs_received_total": received, "safety_denied_total": denied, "jobs_completed_total": completed,
+            "jobs_dispatched_total": dispatched}

@@ -123,6 +123,13 @@ class CordumPlan(C.Structure):
     _fields_ = [("n_slots", C.c_uint32), ("n_jobs", C.c_uint32), ("offsets", C.c_void_p), ("jobs", C.c_void_p)]
 
 
+class CordumTopicCounts(C.Structure):
+    """cordum_topic_counts: a dispatched batch's jobs counted per TrimSpace(topic) label and outcome column
+    (cordum_batch_topic_counts)."""
+    _fields_ = [("n_rows", C.c_uint32), ("n_jobs", C.c_uint32), ("label_off", C.c_void_p), ("label_bytes", C.c_void_p),
+                ("counts", C.c_void_p)]
+
+
 class CordumEnvelopeCaps(C.Structure):
     _fields_ = [("max_jobs", C.c_uint32), ("max_risk_tags", C.c_uint32), ("max_requires", C.c_uint32), ("max_labels", C.c_uint32),
                 ("arena_bytes", C.c_uint64)]
@@ -155,6 +162,9 @@ PLAN_OUTCOME_NAMES = DEC_NAMES + ["MISSING_TOPIC", "NO_POOL_PREFERRED", "NO_POOL
 # batch subsets: outcome buckets the scheduler retries (include/cordum_b200.h CORDUM_SUBSET_RETRYABLE)
 PLAN_THROTTLE, PLAN_NO_WORKERS, PLAN_POOL_OVERLOADED = 4, 10, 11
 SUBSET_RETRYABLE = (1 << PLAN_THROTTLE) | (1 << PLAN_NO_WORKERS) | (1 << PLAN_POOL_OVERLOADED)
+# topic counts: column k < PLAN_OUTCOMES = outcome k, column COUNT_ROUTED = routed jobs (include/cordum_b200.h CORDUM_COUNT_*)
+COUNT_ROUTED = PLAN_OUTCOMES
+COUNT_COLUMNS = PLAN_OUTCOMES + 1
 REASON_NONE, REASON_RULE, REASON_MISSING_TOPIC, REASON_UNSUPPORTED_TOPIC, REASON_TENANT_MCP = 0, 1, 2, 3, 4
 REASON_EFF_DENIED_TOPIC, REASON_EFF_NOT_ALLOWED_TOPIC, REASON_EFF_MCP, REASON_APPROVAL_GRANTED = 12, 13, 14, 22
 

@@ -413,6 +413,42 @@ int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint
  * encode, subset or free.  NULL (n = 0) when dst's records did not come from cordum_batch_subset. */
 const uint32_t* cordum_batch_parent_index(const cordum_batch* dst, uint32_t* n);
 
+/* ---- per-topic outcome counts of a dispatched batch, for the scheduler's topic-labelled metrics.  The reference's only
+ * metrics are four counter vectors labelled by topic (core/infra/metrics/metrics.go:48-70): jobs_received_total{topic}
+ * (engine.go:239), safety_denied_total{topic} (:333, :344), jobs_completed_total{topic,status} (:217, :404) and
+ * jobs_dispatched_total{topic} (:435).  The label is strings.TrimSpace(req.Topic) (:209, :290).  This call counts a batch's
+ * jobs per (label, plan outcome) on the device, so that a bulk caller can increment those counters without fetching a
+ * record or hashing a topic string per job.
+ *
+ * Columns: column k < CORDUM_PLAN_OUTCOMES counts the jobs whose plan outcome bucket is k (CORDUM_PLAN_*, the same
+ * classification as cordum_batch_plan); column CORDUM_COUNT_ROUTED counts the routed jobs (ROUTE_OK + ROUTE_OK_PREFERRED),
+ * which the plan puts in its worker buckets.  A row's sum over the columns is its number of jobs; the column sums are the
+ * plan's bucket sizes (the routed column: the worker buckets together).
+ * Rows: one per distinct label TrimSpace(raw topic), Go semantics (raw topics that differ only in leading or trailing
+ * white space share a row; "" is a row like any other), in ascending bytewise order of label; rows whose total is zero
+ * are left out.  Labels resolve against the topic dictionary generation the batch was dispatched under: a policy,
+ * routing or workers reload, or a new dictionary generation, after the dispatch does not relabel them.
+ * Valid exactly when cordum_batch_plan is: after cordum_dispatch, or after cordum_batch_wait that follows an async,
+ * resident or tick dispatch (a device encode that fell back to the host encoder included), also on a batch made by
+ * cordum_batch_subset once it has been dispatched; otherwise CORDUM_E_STATE.  CORDUM_E_INVALID for NULL arguments,
+ * CORDUM_E_CUDA on a failed engine, CORDUM_E_STALE for a record that fits no bucket (as cordum_batch_plan).
+ * Synchronous.  The arrays are pinned memory owned by the batch, valid until its next encode, dispatch, topic-counts call
+ * or free; the plan and the counts use separate buffers, so neither call invalidates the other's output.  Device scratch
+ * is O(topic ids of the batch's dictionary generation x CORDUM_COUNT_COLUMNS), grown on first need; when it does not fit
+ * the call is refused with CORDUM_E_CAPACITY and the engine stays usable.  Only the non-zero topic-id rows cross PCIe,
+ * and the host merges them by label: no host work per job.  2 kernel launches per call (0 for an empty batch), counted
+ * by cordum_launch_count; NVTX range "cordum:topic_counts". */
+#define CORDUM_COUNT_ROUTED CORDUM_PLAN_OUTCOMES            /* column 12: ROUTE_OK + ROUTE_OK_PREFERRED */
+#define CORDUM_COUNT_COLUMNS (CORDUM_PLAN_OUTCOMES + 1)     /* 13 */
+typedef struct cordum_topic_counts {
+  uint32_t n_rows;             /* distinct labels among the batch's jobs                                          */
+  uint32_t n_jobs;
+  const uint32_t* label_off;   /* [n_rows + 1]: row r's label is label_bytes[label_off[r] .. label_off[r+1])       */
+  const uint8_t* label_bytes;  /* TrimSpace(raw topic), Go semantics; may hold any byte, NUL too                   */
+  const uint32_t* counts;      /* [n_rows][CORDUM_COUNT_COLUMNS]                                                  */
+} cordum_topic_counts;
+int32_t cordum_batch_topic_counts(cordum_batch* b, cordum_topic_counts* out);
+
 /* Host-side materialisation of what the record indexes (pure functions of rule_idx /
  * reason_code / worker_slot; SURVEY.md A.5).  Each writes a NUL-terminated string
  * into buf (truncating to cap) and returns the full length. */

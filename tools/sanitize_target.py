@@ -1,8 +1,8 @@
 """Small end-to-end run of every kernel for compute-sanitizer (tools/sanitize.sh): policy_kernel, route_kernel (label
 picks, multi-chunk and unsorted pools), worker_chunk / worker_merge, the device encoder, heartbeat ingest, scheduler ticks,
-the wide-mask path, the dispatch plan kernels and the batch subset kernels.  Checks the results against the oracle (the
-plan against a numpy grouping of the records, a subset against its source's records), so a sanitizer-clean run is also a
-correct one."""
+the wide-mask path, the dispatch plan kernels, the batch subset kernels and the topic count kernels.  Checks the results
+against the oracle (the plan against a numpy grouping of the records, a subset against its source's records, the topic
+counts against the records grouped by trimmed topic), so a sanitizer-clean run is also a correct one."""
 import os
 import sys
 
@@ -36,6 +36,26 @@ def plan_same(b, rec, n_slots, what):
     print("ok: plan,", what, flush=True)
 
 
+def counts_same(b, rec, topics, what):
+    """Batch.topic_counts() against the records' plan outcome columns grouped by TrimSpace(raw topic)."""
+    st = rec["route_status"].astype(np.int64)
+    col = np.where((st == wire.ROUTE_OK) | (st == wire.ROUTE_OK_PREFERRED), wire.COUNT_ROUTED,
+                   np.where(st == wire.ROUTE_NOT_ATTEMPTED, rec["sched_decision"].astype(np.int64), 6 + st - wire.ROUTE_MISSING_TOPIC))
+    lab = [oracle_lib.trim_space(t) for t in topics]
+    names = sorted(set(lab))
+    row = {x: i for i, x in enumerate(names)}
+    want = np.zeros((len(names), wire.COUNT_COLUMNS), np.uint32)
+    np.add.at(want, (np.array([row[x] for x in lab], np.int64), col), 1)
+    labels, counts = b.topic_counts()
+    assert labels == names and np.array_equal(counts, want), what
+    print("ok: topic counts,", what, flush=True)
+
+
+def topics_of(env):
+    t = env.cols["topic"][:env.n_jobs]
+    return [bytes(env.arena[int(o):int(o) + int(n)]) for o, n in zip(t["off"], t["len"])]
+
+
 def subset_same(b, dst, rec, what):
     """A subset by outcome and one by list (across a tile edge), dispatched: each job decides as its source job did."""
     st = rec["route_status"]
@@ -63,6 +83,7 @@ def main():
         rec = b.encode(cfg.jobs).dispatch(mode)
         same(rec, o.eval(cfg.jobs, mode), "c2 host-encode mode %d" % mode)
         plan_same(b, rec, cfg.workers.n_workers, "c2 mode %d" % mode)   # 1,012 buckets: two radix passes
+        counts_same(b, rec, topics_of(cfg.jobs), "c2 mode %d" % mode)
     same(b.encode_device(cfg.jobs).dispatch(), o.eval(cfg.jobs), "c2 device-encode")
     # heartbeat deltas + refresh
     rng = np.random.default_rng(3)
