@@ -171,8 +171,8 @@ struct cordum_batch {
   const uint32_t* d_slot_of = nullptr;   // device slot_of of records produced on the device (encoder work array or d_sub_idx)
   // cordum_batch_subset, when this batch is the destination
   bool is_subset = false;        // the records are a subset of another batch's: h_parent is valid
-  DevBuf d_sub_idx;              // [max_jobs] slot_of, then [max_jobs] parent index (allocated on first use)
-  DevBuf d_subset;               // scratch of the call (subset_batch), grown on first need
+  DevBuf d_sub_idx;              // [max_jobs] slot_of, then [max_jobs] parent index (allocated on first use; a merge uses the first half)
+  DevBuf d_subset;               // scratch of the call (subset_batch, merge_batch), grown on first need
   uint32_t* h_parent = nullptr;  // pinned [max_jobs]: source job index of each job
   uint32_t last_mode = 0;
   bool last_copy_out = false, timed = true;
@@ -1295,6 +1295,108 @@ int subset_batch(cordum_engine* e, cordum_batch* src, uint32_t mask, const uint3
   *n_out = m;
   return CORDUM_OK;
 }
+
+// cordum_batch_merge once the arguments, the three batches' states and dst's job capacity have been checked.  Scratch of
+// dst (32-bit words): key a [n_a] | key b [n_b] | wloc a [n_sel_a] | wloc b [n_sel_b] | wcnt a, wcnt b [sel tiles] | totals [2].
+int merge_batch(cordum_engine* e, cordum_batch* a, cordum_batch* b, cordum_batch* dst) {
+  MergeParams P{};
+  const uint32_t T = CORDUM_SUBSET_TILE, m = a->n + b->n;
+  if (a->n && b->n && a->wide_words != b->wide_words) {
+    g_err = "the two batches' records have different wide-mask widths: encode them again";
+    return CORDUM_E_STALE;
+  }
+  P.ww = a->n ? a->wide_words : b->n ? b->wide_words : 0u;   // an empty source imposes no width
+  size_t words = 2, extra = 0;
+  cordum_batch* src[2] = {a, b};
+  for (int k = 0; k < 2; ++k) {
+    MergeSource& S = P.s[k];
+    JobRecords R;
+    device_records(src[k], R);
+    S.job = R.job; S.route = R.route; S.wide = R.wide; S.sel_jobs = R.sel_jobs; S.sel_extra = R.sel_extra;
+    S.n = src[k]->n;
+    S.n_sel = R.n_sel_jobs;
+    S.n_tiles = (uint32_t)(((uint64_t)S.n + T - 1) / T);
+    S.n_sel_tiles = (uint32_t)(((uint64_t)S.n_sel + T - 1) / T);
+    words += (size_t)S.n + S.n_sel + S.n_sel_tiles;
+    // the source's extra words, without its leading 0 word (host encoder layout: sel_words = 2 n_sel + 1 + extra)
+    if (S.n_sel) extra += src[k]->sel_words - 2 * (size_t)S.n_sel - 1;
+  }
+  P.m_sel = P.s[0].n_sel + P.s[1].n_sel;
+  const uint64_t wide_need = (uint64_t)m * P.ww, sel_need = P.m_sel ? 2ull * P.m_sel + 1 + extra : 0;
+  cudaError_t ae = dst->d_subset.reserve((words + words / 4) * 4);
+  if (ae == cudaSuccess) ae = dst->d_sub_idx.reserve(2 * (size_t)dst->max_jobs * 4);   // the subset's size: neither call reallocates it
+  if (ae != cudaSuccess) {
+    cudaGetLastError();
+    g_err = "out of memory for the scratch of a merge of " + std::to_string(m) + " jobs";
+    return CORDUM_E_CAPACITY;
+  }
+  uint32_t* w = (uint32_t*)dst->d_subset.p;
+  P.s[0].key = w; P.s[1].key = w + P.s[0].n;
+  P.s[0].wloc = P.s[1].key + P.s[1].n; P.s[1].wloc = P.s[0].wloc + P.s[0].n_sel;
+  P.s[0].wcnt = P.s[1].wloc + P.s[1].n_sel; P.s[1].wcnt = P.s[0].wcnt + P.s[0].n_sel_tiles;
+  P.totals = P.s[1].wcnt + P.s[1].n_sel_tiles;
+  cudaStream_t s = dst->stream;
+  {
+    // e->mu: a dictionary upload on another thread must not replace the tenant-class table between here and the launch
+    std::lock_guard<std::mutex> g(e->mu);
+    std::lock_guard<std::mutex> gh(e->host->mutex());
+    if (a->epoch != e->host->epoch() || b->epoch != e->host->epoch()) {
+      g_err = "tables were reloaded after a source batch was encoded: encode again";
+      return CORDUM_E_STALE;
+    }
+    if (m) {
+      int rc = sync_dicts(e);   // the tenant classes of the sources' epoch, also on an engine that never encoded on the device
+      if (rc) return rc;
+      P.tenant_class = e->et.tenant_class;
+      P.tenant_classes = e->et.tenant_classes;
+    }
+    if (wide_need > dst->wide_cap || sel_need > dst->sel_cap) {
+      // Grown with the encoders' headroom, as for a subset; both new pairs are allocated before either old one is released,
+      // so a refusal leaves dst as it was.
+      const uint64_t wide_want = wide_need > dst->wide_cap ? P.ww * std::min<uint64_t>(dst->max_jobs, std::max<uint64_t>(1024, (uint64_t)m + m / 4)) : 0;
+      const uint64_t sel_want = sel_need > dst->sel_cap ? std::max<uint64_t>(sel_need + sel_need / 4, 1024) : 0;
+      NewPair nw, ns;
+      if ((wide_want && !nw.alloc(wide_want * 8)) || (sel_want && !ns.alloc(sel_want * 4))) {
+        nw.release();
+        ns.release();
+        g_err = "out of memory for the wide-mask rows or the selective list of a merge of " + std::to_string(m) + " jobs";
+        return CORDUM_E_CAPACITY;
+      }
+      if (wide_want) {
+        if (dst->h_wide) cudaFreeHost(dst->h_wide);
+        if (dst->d_wide) cudaFree(dst->d_wide);
+        dst->h_wide = (uint64_t*)nw.h; dst->d_wide = (uint64_t*)nw.d; dst->wide_cap = wide_want;
+      }
+      if (sel_want) {
+        if (dst->h_sel) cudaFreeHost(dst->h_sel);
+        if (dst->d_sel) cudaFree(dst->d_sel);
+        dst->h_sel = (uint32_t*)ns.h; dst->d_sel = (uint32_t*)ns.d; dst->sel_cap = sel_want;
+      }
+      e->tables_gen++;   // captured tick graphs bake the batch's pointers in
+    }
+    P.djob = (JobRec*)dst->d_cols;
+    P.droute = (RouteRec*)(dst->d_cols + (size_t)m * sizeof(JobRec));
+    P.dwide = dst->d_wide;
+    P.dsel = dst->d_sel;
+    P.dslot_of = (uint32_t*)dst->d_sub_idx.p;
+    CK(launch_merge(P, s), "merge kernels");
+    e->launches += merge_launches(P);
+  }
+  CK(cudaStreamSynchronize(s), "merge");
+  dst->n = m;
+  dst->epoch = a->epoch;
+  dst->wide_words = P.ww;
+  dst->n_sel_jobs = P.m_sel;
+  dst->sel_words = (uint32_t)sel_need;
+  dst->d_slot_of = P.dslot_of;
+  dst->env = nullptr;
+  if (dst->h_fallback) *dst->h_fallback = 0;   // records produced here never go back to the host encoder
+  dst->encoded = dst->resident = dst->device_encoded = true;
+  dst->host_records_valid = false;
+  dst->results_ready = false;
+  dst->is_subset = false;
+  return CORDUM_OK;
+}
 }  // namespace
 
 // ============================================================ C ABI
@@ -1883,6 +1985,34 @@ const uint32_t* cordum_batch_parent_index(const cordum_batch* dst, uint32_t* n) 
   const bool ok = dst && dst->is_subset;
   if (n) *n = ok ? dst->n : 0;
   return ok ? dst->h_parent : nullptr;
+}
+int32_t cordum_batch_merge(cordum_batch* a, cordum_batch* b, cordum_batch* dst) {
+  cordum::NvtxRange nvtx_("cordum:merge");
+  if (!a || !b || !dst) { g_err = "null argument"; return CORDUM_E_INVALID; }
+  if (dst == a || dst == b) { g_err = "the merge must go to another batch than its sources"; return CORDUM_E_INVALID; }
+  if (a->e != b->e || a->e != dst->e) { g_err = "the batches belong to different engines"; return CORDUM_E_INVALID; }
+  cordum_engine* e = a->e;
+  if (e->failed) { g_err = "engine failed earlier: " + e->fail_msg; return CORDUM_E_CUDA; }
+  for (const cordum_batch* x : {a, b})
+    if (!x->encoded || !x->resident || x->pending || x->enc_inflight || x->tick_pending) {
+      g_err = "a source batch's records are not complete on the device: wait for its encode, dispatch or tick, or dispatch it once";
+      return CORDUM_E_STATE;
+    }
+  {
+    std::lock_guard<std::mutex> gh(e->host->mutex());
+    if (a->epoch != e->host->epoch() || b->epoch != e->host->epoch()) {
+      g_err = "tables were reloaded after a source batch was encoded: encode again";
+      return CORDUM_E_STALE;
+    }
+  }
+  if ((uint64_t)a->n + b->n > dst->max_jobs) {
+    g_err = "the merge has " + std::to_string((uint64_t)a->n + b->n) + " jobs, more than the destination batch holds (" +
+            std::to_string(dst->max_jobs) + ")";
+    return CORDUM_E_CAPACITY;
+  }
+  if (dst->pending || dst->enc_inflight || dst->tick_pending) { int rc = wait(dst); if (rc) return rc; }
+  CK(cudaSetDevice(e->device), "cudaSetDevice");
+  return merge_batch(e, a, b, dst);
 }
 /* copies the decision records still on the device into the pinned result buffer (after a resident run) */
 int32_t cordum_batch_fetch(cordum_batch* b) {

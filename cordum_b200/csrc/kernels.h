@@ -74,6 +74,75 @@ inline uint32_t plan_launches(const PlanParams& P) { return P.n ? 3u * plan_pass
 // ---- batch subsets (subset.cu): a new encoded batch from a chosen subset of an encoded one (cordum_batch_subset)
 #define CORDUM_SUBSET_TILE 2048u   // items (jobs, sorted slots or selective-list entries) per CTA
 #define CORDUM_SUBSET_NONE 0xFFFFFFFFu
+// Tiles of CORDUM_SUBSET_TILE items, shared by the subset (subset.cu) and merge (merge.cu) kernels: 256 threads x 8 items,
+// item = warp * 256 + round * 32 + lane.
+namespace tile2k {
+constexpr uint32_t kThreads = 256, kWarps = kThreads / 32, kItems = CORDUM_SUBSET_TILE / kThreads;
+static_assert(kItems * kThreads == CORDUM_SUBSET_TILE && kItems == 8, "a warp owns 8 rounds of 32 consecutive items");
+
+__device__ __forceinline__ uint32_t item_index(uint32_t tile, uint32_t r) {
+  return tile * CORDUM_SUBSET_TILE + (threadIdx.x >> 5) * (32 * kItems) + r * 32 + (threadIdx.x & 31);
+}
+
+// Exclusive prefix of v over the tile in item order; *total = the tile's sum.  Every thread of the CTA calls it.
+__device__ __forceinline__ void tile_scan(const uint32_t (&v)[kItems], uint32_t (&pre)[kItems], uint32_t* warp_sums, uint32_t* total) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t run = 0;
+#pragma unroll
+  for (uint32_t r = 0; r < kItems; ++r) {
+    uint32_t x = v[r];
+#pragma unroll
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+      if (lane >= o) x += y;
+    }
+    pre[r] = run + x - v[r];
+    run += __shfl_sync(0xFFFFFFFFu, x, 31);
+  }
+  if (lane == 0) warp_sums[warp] = run;
+  __syncthreads();
+  uint32_t before = 0, sum = 0;
+#pragma unroll
+  for (uint32_t w = 0; w < kWarps; ++w) {
+    const uint32_t s = warp_sums[w];
+    before += w < warp ? s : 0u;
+    sum += s;
+  }
+  __syncthreads();   // warp_sums is reused by the next call
+#pragma unroll
+  for (uint32_t r = 0; r < kItems; ++r) pre[r] += before;
+  *total = sum;
+}
+
+// Exclusive prefix of row[0 .. n) in place (one CTA, every thread calls it); returns the sum.
+__device__ __forceinline__ uint32_t tiles_scan(uint32_t* row, uint32_t n, uint32_t* warp_sums) {
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t carry = 0;
+  for (uint32_t t0 = 0; t0 < n; t0 += kThreads) {
+    const uint32_t t = t0 + threadIdx.x;
+    const uint32_t v = t < n ? row[t] : 0u;
+    uint32_t x = v;
+#pragma unroll
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_sums[warp] = x;
+    __syncthreads();
+    uint32_t before = 0, sum = 0;
+#pragma unroll
+    for (uint32_t w = 0; w < kWarps; ++w) {
+      const uint32_t s = warp_sums[w];
+      before += w < warp ? s : 0u;
+      sum += s;
+    }
+    __syncthreads();
+    if (t < n) row[t] = carry + before + x - v;
+    carry += sum;
+  }
+  return carry;
+}
+}  // namespace tile2k
 struct SubsetParams {
   // source batch (device)
   uint32_t n;                      // jobs
@@ -109,6 +178,38 @@ cudaError_t launch_subset_count(const SubsetParams& P, cudaStream_t s);
 cudaError_t launch_subset_gather(const SubsetParams& P, cudaStream_t s);
 inline uint32_t subset_count_launches(const SubsetParams& P) { return P.n ? 3u : 0u; }
 inline uint32_t subset_launches(const SubsetParams& P) { return P.n ? 4u : 0u; }
+
+// ---- batch merges (merge.cu): one encoded batch from two of the same table epoch (cordum_batch_merge)
+struct MergeSource {               // a source batch (device)
+  const JobRec* job;
+  const RouteRec* route;
+  const uint64_t* wide;            // [n][MergeParams.ww] or null
+  const uint2* sel_jobs;           // the selective list (tables.h JobRecords) or null
+  const uint32_t* sel_extra;
+  uint32_t n, n_sel;
+  uint32_t n_tiles, n_sel_tiles;   // tiles of its n sorted slots and of its n_sel entries
+  // scratch (device)
+  uint32_t* key;                   // [n] the encoders' sort key of each sorted record
+  uint32_t* wloc;                  // [n_sel] per entry: extra words of the tile's entries before it
+  uint32_t* wcnt;                  // [n_sel_tiles] per tile: its extra words; exclusive prefix over the tiles after the scan
+};
+struct MergeParams {
+  MergeSource s[2];                // a, b: b's jobs follow a's
+  const uint8_t* tenant_class;     // device, per tenant id (EncodeTables.tenant_class)
+  uint32_t tenant_classes;
+  uint32_t ww;                     // wide-row width of the non-empty sources
+  uint32_t* totals;                // [2] extra words of a's and of b's entries
+  // destination batch (device)
+  JobRec* djob;
+  RouteRec* droute;
+  uint64_t* dwide;                 // [n_a + n_b][ww]
+  uint32_t* dsel;                  // [2 m_sel] {slot, x}, then the extra words
+  uint32_t m_sel;                  // = a's n_sel + b's n_sel
+  uint32_t* dslot_of;              // [n_a + n_b]
+};
+// key -> scan -> gather, all on stream s
+cudaError_t launch_merge(const MergeParams& P, cudaStream_t s);
+inline uint32_t merge_launches(const MergeParams& P) { return P.s[0].n + P.s[1].n ? 3u : 0u; }
 
 // ---- per-topic outcome counts (counts.cu): a dispatched batch's jobs counted per (topic id, outcome column)
 #define CORDUM_COUNT_TILE 2048u     // sorted records per CTA of the count kernel

@@ -23,43 +23,12 @@
 
 namespace {
 
-constexpr uint32_t kThreads = 256, kWarps = kThreads / 32, kItems = CORDUM_SUBSET_TILE / kThreads;
-static_assert(kItems * kThreads == CORDUM_SUBSET_TILE && kItems == 8, "a warp owns 8 rounds of 32 consecutive items");
+using tile2k::kThreads;
+using tile2k::kWarps;
+using tile2k::kItems;
+using tile2k::item_index;
+using tile2k::tile_scan;
 constexpr uint32_t kNone = CORDUM_SUBSET_NONE;
-
-__device__ __forceinline__ uint32_t item_index(uint32_t tile, uint32_t r) {
-  return tile * CORDUM_SUBSET_TILE + (threadIdx.x >> 5) * (32 * kItems) + r * 32 + (threadIdx.x & 31);
-}
-
-// Exclusive prefix of v over the tile in item order; *total = the tile's sum.  Every thread of the CTA calls it.
-__device__ __forceinline__ void tile_scan(const uint32_t (&v)[kItems], uint32_t (&pre)[kItems], uint32_t* warp_sums, uint32_t* total) {
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t run = 0;
-#pragma unroll
-  for (uint32_t r = 0; r < kItems; ++r) {
-    uint32_t x = v[r];
-#pragma unroll
-    for (uint32_t o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(FULL, x, o);
-      if (lane >= o) x += y;
-    }
-    pre[r] = run + x - v[r];
-    run += __shfl_sync(FULL, x, 31);
-  }
-  if (lane == 0) warp_sums[warp] = run;
-  __syncthreads();
-  uint32_t before = 0, sum = 0;
-#pragma unroll
-  for (uint32_t w = 0; w < kWarps; ++w) {
-    const uint32_t s = warp_sums[w];
-    before += w < warp ? s : 0u;
-    sum += s;
-  }
-  __syncthreads();   // warp_sums is reused by the next call
-#pragma unroll
-  for (uint32_t r = 0; r < kItems; ++r) pre[r] += before;
-  *total = sum;
-}
 
 // Outcome bucket of a decision record (include/cordum_b200.h CORDUM_PLAN_*), or NONE for a routed job.
 __device__ __forceinline__ uint32_t outcome_of(uint4 rec) {
@@ -167,30 +136,7 @@ __global__ void __launch_bounds__(kThreads) subset_scan_kernel(SubsetParams P) {
   __shared__ uint32_t warp_sums[kWarps];
   uint32_t* row = blockIdx.x == 0 ? P.jcnt : blockIdx.x == 1 ? P.scnt : blockIdx.x == 2 ? P.ecnt : P.wcnt;
   const uint32_t n = blockIdx.x < 2 ? P.n_tiles : P.n_sel_tiles;
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t carry = 0;
-  for (uint32_t t0 = 0; t0 < n; t0 += kThreads) {
-    const uint32_t t = t0 + threadIdx.x;
-    const uint32_t v = t < n ? row[t] : 0u;
-    uint32_t x = v;
-#pragma unroll
-    for (uint32_t o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(FULL, x, o);
-      if (lane >= o) x += y;
-    }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    uint32_t before = 0, sum = 0;
-#pragma unroll
-    for (uint32_t w = 0; w < kWarps; ++w) {
-      const uint32_t s = warp_sums[w];
-      before += w < warp ? s : 0u;
-      sum += s;
-    }
-    __syncthreads();
-    if (t < n) row[t] = carry + before + x - v;
-    carry += sum;
-  }
+  const uint32_t carry = tile2k::tiles_scan(row, n, warp_sums);
   if (threadIdx.x == 0) P.totals[blockIdx.x] = carry;
 }
 

@@ -170,6 +170,14 @@ class Batch:
         dst._env = None   # dst holds no envelopes: MCP reasons quote the canonical spelling
         return m.value
 
+    def merge(self, other: "Batch", dst: "Batch") -> int:
+        """Make `dst` the encoded batch of this batch's jobs followed by `other`'s (cordum_batch_merge), on the device: its
+        records are those a host encode of both batches' envelopes, this one's first, would give.  `other` may be this
+        batch.  Returns dst's job count."""
+        self.eng._ck(self.L.cordum_batch_merge(self.h, other.h, dst.h))
+        dst._env = None   # dst holds no envelopes: MCP reasons quote the canonical spelling
+        return dst.size
+
     def parent_index(self) -> np.ndarray:
         """This batch's job i -> the source batch's job index, when its records came from Batch.subset (else empty).  A
         view of library memory, valid until this batch's next encode, subset or free."""

@@ -413,6 +413,38 @@ int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint
  * encode, subset or free.  NULL (n = 0) when dst's records did not come from cordum_batch_subset. */
 const uint32_t* cordum_batch_parent_index(const cordum_batch* dst, uint32_t* n);
 
+/* ---- batch merges: the retries and the new arrivals of a heartbeat epoch as one batch.  Redelivered jobs (RetryAfter,
+ * engine.go:303-315, 393-402) go through checkSafetyDecision and PickSubject again, together with the jobs that arrived
+ * since; cordum_batch_merge builds one encoded batch from two encoded batches of the same table epoch (typically a
+ * cordum_batch_subset of the retryable jobs and a device encode of the new arrivals), so that both take one dispatch or
+ * one cordum_tick_async instead of two, and nothing is encoded again or crosses PCIe.
+ *
+ * Result: dst becomes an encoded batch of n_a + n_b jobs, resident on the device, whose records equal bit for bit what
+ * cordum_encode makes of a's envelopes followed by b's: job i < n_a is a's job i, job n_a + i is b's job i (JobRec.orig of
+ * b's records moves up by n_a); the records are the stable merge of a's and b's sorted records by the encoders' key
+ * (topic id x tenant classes + tenant class), a before b on equal keys; wide rows follow their records; the selective
+ * list is {merged slot, x} per entry in ascending slot with the extra words re-packed in entry order behind the leading
+ * 0 word; slot_of is set for every job; the epoch is the sources'.  (The device encoder orders the jobs of one key as
+ * its threads claim slots; a merge keeps each source's order, so with a device-encoded source the order within a key is
+ * that one, while every job's records are still the host encoder's bit for bit.)  a == b is allowed (dst holds its jobs twice); either
+ * source may be empty (an empty source imposes no wide-row width).  dst keeps no pointer to a or b (either may be freed
+ * or re-encoded) and never falls back to the host encoder.  Every dispatch form (blocking, async, resident,
+ * cordum_tick_async), cordum_batch_plan, cordum_batch_topic_counts, cordum_batch_subset, another cordum_batch_merge,
+ * cordum_batch_records, cordum_reason* (MCP values in their canonical spelling) and cordum_subject work on it;
+ * cordum_batch_parent_index(dst) is NULL (n = 0), since the job mapping above is fixed.
+ * Each source's records must be complete on the device, as for cordum_batch_subset's list form: a device encode that has
+ * been waited for without falling back, a batch dispatched at least once and not in flight (waited for after an async
+ * dispatch or a tick, a device encode that fell back included), or a subset or merge destination.
+ * Synchronous; waits for dst first if dst is in flight.  3 kernel launches (0 when both sources are empty), counted by
+ * cordum_launch_count; NVTX range "cordum:merge".
+ * Refusals, after each of which the engine stays usable: CORDUM_E_INVALID for NULL arguments, dst == a or dst == b, or
+ * batches of different engines.  CORDUM_E_STATE for a source that is a host-encoded batch never dispatched, or in flight
+ * (an encode, dispatch or tick not yet waited for).  CORDUM_E_STALE when either source's epoch is not the current table
+ * epoch (a policy, routing or workers reload, or a new dictionary generation, after its encode; heartbeats keep the
+ * epoch).  CORDUM_E_CAPACITY when n_a + n_b exceeds dst's max_jobs (checked on the host before any device work), or when
+ * the scratch or dst's wide rows or selective list cannot be grown; dst is then left exactly as it was. */
+int32_t cordum_batch_merge(cordum_batch* a, cordum_batch* b, cordum_batch* dst);
+
 /* ---- per-topic outcome counts of a dispatched batch, for the scheduler's topic-labelled metrics.  The reference's only
  * metrics are four counter vectors labelled by topic (core/infra/metrics/metrics.go:48-70): jobs_received_total{topic}
  * (engine.go:239), safety_denied_total{topic} (:333, :344), jobs_completed_total{topic,status} (:217, :404) and

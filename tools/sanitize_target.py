@@ -1,8 +1,9 @@
 """Small end-to-end run of every kernel for compute-sanitizer (tools/sanitize.sh): policy_kernel, route_kernel (label
 picks, multi-chunk and unsorted pools), worker_chunk / worker_merge, the device encoder, heartbeat ingest, scheduler ticks,
-the wide-mask path, the dispatch plan kernels, the batch subset kernels and the topic count kernels.  Checks the results
-against the oracle (the plan against a numpy grouping of the records, a subset against its source's records, the topic
-counts against the records grouped by trimmed topic), so a sanitizer-clean run is also a correct one."""
+the wide-mask path, the dispatch plan kernels, the batch subset and merge kernels and the topic count kernels.  Checks the
+results against the oracle (the plan against a numpy grouping of the records, a subset against its source's records, a
+merge against a host encode of both sources' envelopes and their records, the topic counts against the records grouped
+by trimmed topic), so a sanitizer-clean run is also a correct one."""
 import os
 import sys
 
@@ -69,6 +70,28 @@ def subset_same(b, dst, rec, what):
         same(dst.dispatch().copy()[:m], rec[parent], "subset (%s), %s" % (sorted(kw)[0], what))
 
 
+def merge_same(e, b, env, what):
+    """b merged with a host encode of its first third, then with itself: records, selective list and wide rows equal a host
+    encode of both envelope lists, and each job decides as it did in its source."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_batch_subset as tbs
+
+    env = env if isinstance(env, wire.EnvelopeBatch) else wire.EnvelopeBatch.from_jobs(env)
+    n = env.n_jobs
+    k = max(1, n // 3)
+    part, dst = e.batch(k), e.batch(2 * n)
+    part.encode(env.slice(0, k)).dispatch()
+    for other, idx in ((part, np.arange(k)), (b, np.arange(n))):
+        assert b.merge(other, dst) == n + len(idx), what
+        job, route, slot = dst.records()
+        hjob, hroute, hslot, hsel, hwide = tbs.host_records_of(e, tbs.take(env, np.concatenate([np.arange(n), idx])))
+        assert job.tobytes() == hjob.tobytes() and route.tobytes() == hroute.tobytes() and np.array_equal(slot, hslot), what
+        assert np.array_equal(tbs.side(dst, 0), hsel) and np.array_equal(tbs.side(dst, 1), hwide), what
+        same(dst.dispatch().copy(), np.concatenate([b.results().copy(), other.results().copy()]), "merge, %s" % what)
+    part.free()
+    dst.free()
+
+
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     light = len(sys.argv) > 2 and sys.argv[2] == "light"   # racecheck serialises everything: smaller pools, fewer phases
@@ -97,6 +120,7 @@ def main():
     same(b.encode(cfg.jobs).dispatch(), o.eval(cfg.jobs), "after heartbeat deltas")
     dst = e.batch(n)
     subset_same(b, dst, b.results().copy(), "c2")
+    merge_same(e, b, cfg.jobs, "c2")
     # one big pool: multi-chunk merge (1300) and beyond the sort buffer (9000)
     for size in ((1300,) if light else (1300, 9000)):
         routing = {"topics": {"job.w.go": ["big"]}, "pools": {"big": {}}}
@@ -121,6 +145,7 @@ def main():
     bw = e.batch(len(jobs))
     same(bw.encode(jobs).dispatch(), o3.eval(jobs), "wide masks")
     subset_same(bw, e.batch(len(jobs)), bw.results().copy(), "wide masks")
+    merge_same(e, bw, jobs, "wide masks")
     o3.close()
     # selective placement pairs: the subset re-packs the selective list and its extra words
     import test_selective_differential as tsd
@@ -132,6 +157,7 @@ def main():
     e.load_workers(workers)
     bs = e.batch(len(jobs))
     subset_same(bs, e.batch(len(jobs)), bs.encode(jobs).dispatch().copy(), "selective pairs")
+    merge_same(e, bs, jobs, "selective pairs")
     # scheduler ticks on the c2 tables
     e.load_policy(cfg.policy, "san2")
     e.load_routing(cfg.routing)
