@@ -22,7 +22,7 @@ API = [
     "cordum_batch_alloc", "cordum_batch_free", "cordum_encode", "cordum_encode_device", "cordum_envelopes_alloc",
     "cordum_envelopes_free", "cordum_host_fallbacks", "cordum_batch_records", "cordum_dispatch",
     "cordum_dispatch_async", "cordum_batch_wait", "cordum_dispatch_resident", "cordum_dispatch_resident_async", "cordum_batch_fetch", "cordum_batch_stream",
-    "cordum_batch_size", "cordum_batch_results", "cordum_batch_timing", "cordum_batch_kernel_times", "cordum_batch_plan", "cordum_batch_topic_counts", "cordum_batch_subset", "cordum_batch_parent_index", "cordum_batch_merge", "cordum_rule_id", "cordum_reason", "cordum_reason_flavor", "cordum_batch_snapshot", "cordum_batch_policy_gen", "cordum_policy_generation", "cordum_frontend_cache_stats", "cordum_rule_id_at", "cordum_rule_constraints_json_at", "cordum_rule_remediations_json_at",
+    "cordum_batch_size", "cordum_batch_results", "cordum_batch_timing", "cordum_batch_kernel_times", "cordum_batch_plan", "cordum_batch_topic_counts", "cordum_batch_responses", "cordum_batch_subset", "cordum_batch_parent_index", "cordum_batch_merge", "cordum_rule_id", "cordum_reason", "cordum_reason_flavor", "cordum_batch_snapshot", "cordum_batch_policy_gen", "cordum_policy_generation", "cordum_frontend_cache_stats", "cordum_rule_id_at", "cordum_rule_constraints_json_at", "cordum_rule_remediations_json_at",
     "cordum_subject", "cordum_rule_constraints_json", "cordum_rule_remediations_json", "cordum_stats",
     "cordum_launch_count", "cordum_frontend_create", "cordum_frontend_destroy", "cordum_frontend_submit", "cordum_frontend_submit_many", "cordum_frontend_stats", "cordum_frontend_loadgen",
     "cordum_test_glob", "cordum_test_trim", "cordum_test_normalize_decision",
@@ -89,6 +89,7 @@ def load() -> C.CDLL:
     L.cordum_batch_kernel_times.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
     L.cordum_batch_plan.argtypes = [vp, C.POINTER(wire.CordumPlan)]
     L.cordum_batch_topic_counts.argtypes = [vp, C.POINTER(wire.CordumTopicCounts)]
+    L.cordum_batch_responses.argtypes = [vp, u32, C.POINTER(wire.CordumResponses)]
     L.cordum_batch_subset.argtypes = [vp, u32, vp, u32, vp, C.POINTER(u32)]
     L.cordum_batch_parent_index.argtypes = [vp, C.POINTER(u32)]
     L.cordum_batch_parent_index.restype = vp

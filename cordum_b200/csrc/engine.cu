@@ -187,6 +187,11 @@ struct cordum_batch {
   DevBuf d_counts;               // cordum_batch_topic_counts scratch (count_batch), grown on first need
   uint32_t* h_counts = nullptr;  // pinned: the copied topic rows, then the output (counts | label offsets | label bytes)
   size_t h_counts_cap = 0;       // 32-bit words
+  DevBuf d_resp;                 // cordum_batch_responses scratch (responses_batch), grown on first need
+  uint32_t* h_resp = nullptr;    // pinned: the class count, classes, offsets, jobs, then the two text offset arrays
+  size_t h_resp_cap = 0;         // 32-bit words
+  uint8_t* h_resp_text = nullptr;   // pinned: the reasons' and rule ids' bytes
+  size_t h_resp_text_cap = 0;
   uint2* d_route = nullptr;           // [0].x = count, [2..] = compacted list of dispatchable jobs {slot, head}
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr, ev2 = nullptr, ev3 = nullptr;
@@ -660,6 +665,8 @@ static void batch_release(cordum_batch* b) {   // frees the batch's CUDA resourc
   if (b->h_out) cudaFreeHost(b->h_out);
   if (b->h_plan) cudaFreeHost(b->h_plan);
   if (b->h_counts) cudaFreeHost(b->h_counts);
+  if (b->h_resp) cudaFreeHost(b->h_resp);
+  if (b->h_resp_text) cudaFreeHost(b->h_resp_text);
   if (b->h_parent) cudaFreeHost(b->h_parent);
   if (b->d_out) cudaFree(b->d_out);
   if (b->d_route) cudaFree(b->d_route);
@@ -1168,6 +1175,202 @@ int count_batch(cordum_engine* e, cordum_batch* b, cordum_topic_counts* out) {
   out->counts = h;
   out->label_off = h + cnt.size();
   out->label_bytes = reinterpret_cast<const uint8_t*>(h + cnt.size() + off.size());
+  return CORDUM_OK;
+}
+
+// arg of a record's reason code (the class key of include/cordum_b200.h; responses.cu reason_arg is the device's copy).
+uint32_t reason_arg(uint32_t code, const JobRec& j) {
+  if (code == CORDUM_REASON_EFF_DENIED_TOPIC || code == CORDUM_REASON_EFF_NOT_ALLOWED_TOPIC) return j.topic;
+  if (code >= CORDUM_REASON_TENANT_MCP && code < CORDUM_REASON_TENANT_MCP + 8) return j.mcp[(code - CORDUM_REASON_TENANT_MCP) >> 1];
+  if (code >= CORDUM_REASON_EFF_MCP && code < CORDUM_REASON_EFF_MCP + 8) return j.mcp[(code - CORDUM_REASON_EFF_MCP) >> 1];
+  return 0;
+}
+bool mcp_reason(uint32_t code) {
+  return (code >= CORDUM_REASON_TENANT_MCP && code < CORDUM_REASON_TENANT_MCP + 8) ||
+         (code >= CORDUM_REASON_EFF_MCP && code < CORDUM_REASON_EFF_MCP + 8);
+}
+
+// The reason text of a record of batch b (kernel.go:172,175,221,225; safety_policy.go:410,413; engine.go:500), from its
+// reason code, rule index and reason_arg.  With env, an MCP reason quotes the request's own spelling of job's value (%q of
+// the trimmed label value, as the reference does); without it the canonical (trimmed, case-folded) form the dictionaries
+// keep.  Called with the host mutex held.  False when that canonical form is gone (the value dictionaries were rebuilt
+// since the batch was encoded).
+bool render_reason(cordum_engine* e, const cordum_batch* b, uint32_t code, int32_t rule_idx, uint32_t arg, uint32_t flavor,
+                   const cordum_envelopes* env, uint32_t job, std::string& s) {
+  static const char* fields[4] = {"server", "tool", "resource", "action"};
+  s.clear();
+  if (code == CORDUM_REASON_RULE) {
+    // the policy the batch was dispatched under, not whatever is in force by now
+    if (b->text && rule_idx >= 0 && (size_t)rule_idx < b->text->rules.size()) s = b->text->rules[rule_idx].reason;
+  } else if (code == CORDUM_REASON_MISSING_TOPIC) s = "missing topic";
+  else if (code == CORDUM_REASON_UNSUPPORTED_TOPIC) s = "unsupported topic";
+  else if (code == CORDUM_REASON_APPROVAL_GRANTED) s = "approval granted";
+  else if (code == CORDUM_REASON_EFF_DENIED_TOPIC || code == CORDUM_REASON_EFF_NOT_ALLOWED_TOPIC) {
+    std::string topic((b->ttext && arg < b->ttext->size()) ? cordum::trim_space((*b->ttext)[arg]) : sv());
+    const char* tail = code == CORDUM_REASON_EFF_DENIED_TOPIC ? " denied by effective config" : " not allowed by effective config";
+    // kernel.go:221,225 print '%s'; the gateway's copy of the evaluator prints %q (policy_bundles.go:1207,1211)
+    s = "topic " + (flavor == CORDUM_REASON_FLAVOR_GATEWAY ? cordum::go_quote(topic) : "'" + topic + "'") + tail;
+  } else if (mcp_reason(code)) {
+    uint32_t k = code >= CORDUM_REASON_EFF_MCP ? code - CORDUM_REASON_EFF_MCP : code - CORDUM_REASON_TENANT_MCP;
+    int f = (int)(k >> 1);
+    if (!env && b->epoch != e->host->epoch()) return false;   // the value dictionaries were rebuilt since: only the envelopes still know
+    std::string v = env ? cordum::mcp_request_value(env, job, f) : e->host->mcp_value_string(f, arg);
+    s = std::string("mcp ") + fields[f] + " " + cordum::go_quote(v) + ((k & 1) ? " not allowed" : " denied");
+  }
+  return true;
+}
+
+// A pinned buffer of the batch grown to at least `count` elements; false (buffer released) when it does not fit.
+template <class T>
+bool pinned_reserve(T*& p, size_t& cap, size_t count) {
+  if (count <= cap) return true;
+  if (p) cudaFreeHost(p);
+  p = nullptr;
+  cap = 0;
+  const size_t want = std::max<size_t>(count + count / 4, 64);
+  if (cudaHostAlloc((void**)&p, want * sizeof(T), cudaHostAllocDefault) != cudaSuccess) {
+    cudaGetLastError();   // an allocation that does not fit is this call's problem, not a sticky engine failure
+    p = nullptr;
+    return false;
+  }
+  cap = want;
+  return true;
+}
+
+// cordum_batch_responses on a batch whose records are complete in d_out.  Device scratch (32-bit words): keys x 2 [2n
+// each] | vals x 2 [n each] | jflag, sloc, perm, start, size [n each] | classes [4n] | offsets [n + 1] | jobs [n] | counts
+// [256][tiles] | totals [256] | hcnt, jcnt, ccnt [tiles each] | head [2].  Pinned: head [2] | classes [4m] | offsets
+// [m + 1] | jobs [n] | reason offsets [m + 1] | rule id offsets [m + 1]; the text bytes in an arena of their own.
+int responses_batch(cordum_engine* e, cordum_batch* b, uint32_t flavor, cordum_responses* out) {
+  constexpr uint32_t T = CORDUM_SUBSET_TILE;
+  RespParams P{};
+  JobRecords R;
+  device_records(b, R);
+  P.job = R.job;
+  P.out = reinterpret_cast<const uint4*>(b->d_out);
+  P.n = b->n;
+  P.n_tiles = (uint32_t)(((uint64_t)P.n + T - 1) / T);
+  size_t n_topics;
+  {
+    std::lock_guard<std::mutex> g(e->host->mutex());        // a generation's topic store grows under this lock
+    n_topics = b->ttext ? b->ttext->size() : 0;
+  }
+  auto width = [](uint64_t v) { uint32_t k = 0; while (k < 64 && (v >> k)) ++k; return k; };   // bits that hold 0 .. v
+  const uint64_t n_rules = b->text ? b->text->rules.size() : 0;
+  P.w_rule = width(n_rules);                                   // rule_idx + 1 in 0 .. n_rules
+  P.w_arg = std::max<uint32_t>(16, width(n_topics ? n_topics - 1 : 0));   // MCP value ids are 16-bit
+  const uint32_t key_bits = CORDUM_RESP_FIXED_BITS + P.w_rule + P.w_arg;
+  if (key_bits > 64) {
+    g_err = "the response class key needs " + std::to_string(key_bits) + " bits (" + std::to_string(n_rules) + " rules, " +
+            std::to_string(n_topics) + " topic ids), more than 64";
+    return CORDUM_E_CAPACITY;
+  }
+  P.passes = (key_bits + 7) / 8;
+  const size_t n = P.n, tiles = P.n_tiles, dev_words = n ? 6 * n + 5 * n + 4 * n + (n + 1) + n + 256 * tiles + 256 + 3 * tiles + 2 : 0;
+  const cudaError_t de = dev_words * 4 > b->d_resp.cap ? b->d_resp.reserve(dev_words * 5) : cudaSuccess;   // + 1/4
+  if (de != cudaSuccess || !pinned_reserve(b->h_resp, b->h_resp_cap, 2)) {
+    cudaGetLastError();
+    g_err = "out of memory for the responses of " + std::to_string(n) + " jobs";
+    return CORDUM_E_CAPACITY;
+  }
+  out->n_jobs = P.n;
+  out->policy_gen = b->text ? b->text->gen : 0;
+  if (n == 0) {
+    uint32_t* h = b->h_resp;
+    h[0] = h[1] = 0;   // offsets, reason offsets and rule id offsets: [0]
+    out->n_classes = 0;
+    out->classes = reinterpret_cast<const cordum_response_class*>(h);
+    out->offsets = out->jobs = out->reason_off = out->rule_id_off = h;
+    out->reason_bytes = out->rule_id_bytes = reinterpret_cast<const uint8_t*>(h + 1);
+    return CORDUM_OK;
+  }
+  uint32_t* w = (uint32_t*)b->d_resp.p;
+  P.keys[0] = reinterpret_cast<unsigned long long*>(w);
+  P.keys[1] = reinterpret_cast<unsigned long long*>(w + 2 * n);
+  P.vals[0] = w + 4 * n;
+  P.vals[1] = w + 5 * n;
+  P.jflag = w + 6 * n;
+  P.sloc = w + 7 * n;
+  P.perm = w + 8 * n;
+  P.start = w + 9 * n;
+  P.size = w + 10 * n;
+  P.cls = reinterpret_cast<cordum_response_class*>(w + 11 * n);
+  P.offsets = w + 15 * n;
+  P.jobs = w + 16 * n + 1;
+  P.counts = w + 17 * n + 1;
+  P.totals = P.counts + 256 * tiles;
+  P.hcnt = P.totals + 256;
+  P.jcnt = P.hcnt + tiles;
+  P.ccnt = P.jcnt + tiles;
+  P.head = P.ccnt + tiles;
+  cudaStream_t s = b->stream;
+  CK(cudaMemsetAsync(P.head, 0, 2 * sizeof(uint32_t), s), "responses head");
+  CK(launch_responses(P, s), "response kernels");
+  e->launches += responses_launches(P);
+  CK(cudaMemcpyAsync(b->h_resp, P.head, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s), "D2H response head");
+  CK(cudaStreamSynchronize(s), "responses");
+  if (b->h_resp[1]) {
+    g_err = "a decision record of this batch names a rule or a value outside the tables it was dispatched against: encode and "
+            "dispatch it again";
+    return CORDUM_E_STALE;
+  }
+  const size_t m = b->h_resp[0];
+  const size_t at_cls = 2, at_off = at_cls + 4 * m, at_jobs = at_off + m + 1, at_roff = at_jobs + n, at_ioff = at_roff + m + 1;
+  if (!pinned_reserve(b->h_resp, b->h_resp_cap, at_ioff + m + 1)) {
+    g_err = "out of memory for the " + std::to_string(m) + " response classes of a batch";
+    return CORDUM_E_CAPACITY;
+  }
+  uint32_t* h = b->h_resp;
+  CK(cudaMemcpyAsync(h + at_cls, P.cls, m * sizeof(cordum_response_class), cudaMemcpyDeviceToHost, s), "D2H response classes");
+  CK(cudaMemcpyAsync(h + at_off, P.offsets, (m + 1) * 4, cudaMemcpyDeviceToHost, s), "D2H response offsets");
+  CK(cudaMemcpyAsync(h + at_jobs, P.jobs, n * 4, cudaMemcpyDeviceToHost, s), "D2H response jobs");
+  CK(cudaStreamSynchronize(s), "response lists");
+  // one reason and one rule id per class (frontend.cpp builds the same per job)
+  auto* cls = reinterpret_cast<cordum_response_class*>(h + at_cls);
+  uint32_t* roff = h + at_roff;
+  uint32_t* ioff = h + at_ioff;
+  std::string text, r;
+  roff[0] = 0;
+  {
+    std::lock_guard<std::mutex> g(e->host->mutex());
+    for (size_t c = 0; c < m; ++c) {
+      cordum_response_class& k = cls[c];
+      if (mcp_reason(k.reason_code) && b->epoch != e->host->epoch()) {
+        g_err = "tables were reloaded after the batch was encoded, and a response quotes an MCP value of the dictionaries it "
+                "was encoded against: encode and dispatch it again";
+        return CORDUM_E_STALE;
+      }
+      // kernel.go:198-215: allow and allow_with_constraints drop the reason, except the approval bypass's (engine.go:500)
+      const bool allow = k.decision == CORDUM_DEC_ALLOW || k.decision == CORDUM_DEC_ALLOW_WITH_CONSTRAINTS;
+      if ((k.reason_code != CORDUM_REASON_NONE && !allow) || k.reason_code == CORDUM_REASON_APPROVAL_GRANTED) {
+        render_reason(e, b, k.reason_code, k.rule_idx, k.arg, flavor, nullptr, k.first_job, r);
+        if (mcp_reason(k.reason_code)) k.flags |= CORDUM_CLASS_QUOTES_VALUE;
+        text += r;
+      }
+      roff[c + 1] = (uint32_t)text.size();
+    }
+    ioff[0] = (uint32_t)text.size();
+    for (size_t c = 0; c < m; ++c) {
+      const cordum_response_class& k = cls[c];
+      if ((k.flags & CORDUM_F_HAS_SNAPSHOT) && b->text && k.rule_idx >= 0 && (size_t)k.rule_idx < b->text->rules.size())
+        text += b->text->rules[k.rule_idx].id;
+      ioff[c + 1] = (uint32_t)text.size();
+    }
+  }
+  for (size_t c = 0; c <= m; ++c) ioff[c] -= roff[m];   // rule id offsets relative to their own arena
+  if (!pinned_reserve(b->h_resp_text, b->h_resp_text_cap, text.size() + 1)) {
+    g_err = "out of memory for the response text of " + std::to_string(m) + " classes";
+    return CORDUM_E_CAPACITY;
+  }
+  std::memcpy(b->h_resp_text, text.data(), text.size());
+  out->n_classes = (uint32_t)m;
+  out->classes = cls;
+  out->offsets = h + at_off;
+  out->jobs = h + at_jobs;
+  out->reason_off = roff;
+  out->reason_bytes = b->h_resp_text;
+  out->rule_id_off = ioff;
+  out->rule_id_bytes = b->h_resp_text + roff[m];
   return CORDUM_OK;
 }
 
@@ -1950,6 +2153,16 @@ int32_t cordum_batch_topic_counts(cordum_batch* b, cordum_topic_counts* out) {
   CK(cudaSetDevice(e->device), "cudaSetDevice");
   return count_batch(e, b, out);
 }
+int32_t cordum_batch_responses(cordum_batch* b, uint32_t flavor, cordum_responses* out) {
+  cordum::NvtxRange nvtx_("cordum:responses");
+  if (!b || !out) { g_err = "null argument"; return CORDUM_E_INVALID; }
+  if (flavor > CORDUM_REASON_FLAVOR_GATEWAY) { g_err = "unknown reason flavor " + std::to_string(flavor); return CORDUM_E_INVALID; }
+  cordum_engine* e = b->e;
+  if (e->failed) { g_err = "engine failed earlier: " + e->fail_msg; return CORDUM_E_CUDA; }
+  if (!b->results_ready) { g_err = "the batch has no completed dispatch: dispatch it, and wait for an asynchronous one, first"; return CORDUM_E_STATE; }
+  CK(cudaSetDevice(e->device), "cudaSetDevice");
+  return responses_batch(e, b, flavor, out);
+}
 int32_t cordum_batch_subset(cordum_batch* src, uint32_t outcome_mask, const uint32_t* jobs, uint32_t n_list, cordum_batch* dst, uint32_t* n_out) {
   cordum::NvtxRange nvtx_("cordum:subset");
   if (!src || !dst || !n_out) { g_err = "null argument"; return CORDUM_E_INVALID; }
@@ -2071,32 +2284,9 @@ int64_t cordum_reason_flavor(cordum_engine* e, const cordum_batch* b, uint32_t j
   if (ensure_host_records(const_cast<cordum_batch*>(b))) return -1;
   std::lock_guard<std::mutex> g(e->host->mutex());
   const cordum_decision& r = b->h_out[job];
-  const uint32_t code = r.reason_code;
   std::string s;
-  static const char* fields[4] = {"server", "tool", "resource", "action"};
-  if (code == CORDUM_REASON_RULE) {
-    // the policy the batch was dispatched under, not whatever is in force by now
-    if (b->text && r.rule_idx >= 0 && (size_t)r.rule_idx < b->text->rules.size()) s = b->text->rules[r.rule_idx].reason;
-  } else if (code == CORDUM_REASON_MISSING_TOPIC) s = "missing topic";
-  else if (code == CORDUM_REASON_UNSUPPORTED_TOPIC) s = "unsupported topic";
-  else if (code == CORDUM_REASON_APPROVAL_GRANTED) s = "approval granted";
-  else if (code == CORDUM_REASON_EFF_DENIED_TOPIC || code == CORDUM_REASON_EFF_NOT_ALLOWED_TOPIC) {
-    const uint32_t tid = b->hr.job[b->hr.slot_of[job]].topic;
-    std::string topic((b->ttext && tid < b->ttext->size()) ? cordum::trim_space((*b->ttext)[tid]) : sv());
-    const char* tail = code == CORDUM_REASON_EFF_DENIED_TOPIC ? " denied by effective config" : " not allowed by effective config";
-    // kernel.go:221,225 print '%s'; the gateway's copy of the evaluator prints %q (policy_bundles.go:1207,1211)
-    s = "topic " + (flavor == CORDUM_REASON_FLAVOR_GATEWAY ? cordum::go_quote(topic) : "'" + topic + "'") + tail;
-  } else if ((code >= CORDUM_REASON_TENANT_MCP && code < CORDUM_REASON_TENANT_MCP + 8) ||
-             (code >= CORDUM_REASON_EFF_MCP && code < CORDUM_REASON_EFF_MCP + 8)) {
-    uint32_t k = code >= CORDUM_REASON_EFF_MCP ? code - CORDUM_REASON_EFF_MCP : code - CORDUM_REASON_TENANT_MCP;
-    int f = (int)(k >> 1);
-    // %q of the request's own spelling (safety_policy.go:410,413) when the caller still holds the envelopes; without
-    // them, the canonical (trimmed, case-folded) form the dictionaries keep
-    if (!env && b->epoch != e->host->epoch()) return -1;   // the value dictionaries were rebuilt since: only the envelopes still know
-    std::string v = env ? cordum::mcp_request_value(env, job, f)
-                        : e->host->mcp_value_string(f, b->hr.job[b->hr.slot_of[job]].mcp[f]);
-    s = std::string("mcp ") + fields[f] + " " + cordum::go_quote(v) + ((k & 1) ? " not allowed" : " denied");
-  }
+  if (!render_reason(e, b, r.reason_code, r.rule_idx, reason_arg(r.reason_code, b->hr.job[b->hr.slot_of[job]]), flavor, env, job, s))
+    return -1;
   return copy_out(s, buf, cap);
 }
 

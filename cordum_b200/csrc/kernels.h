@@ -226,6 +226,34 @@ struct CountParams {
 cudaError_t launch_counts(const CountParams& P, cudaStream_t s);
 inline uint32_t counts_launches(const CountParams& P) { return P.n ? 2u : 0u; }
 
+// ---- batch responses (responses.cu): a dispatched batch's jobs grouped by safety response (cordum_batch_responses)
+// 64-bit class key, from bit 0 up: arg [w_arg] | rule_idx + 1 [w_rule] | reason_code [5] | flags [4] | sched_decision [3] |
+// decision [3].  flags packs APPROVAL_REQUIRED, HAS_SNAPSHOT, CONSTRAINTS into bits 0-2 and APPROVED_BYPASS into bit 3.
+#define CORDUM_RESP_FIXED_BITS 15u
+struct RespParams {
+  const JobRec* job;               // device: the batch's sorted records (topic, orig, mcp)
+  const uint4* out;                // device: its decision records, caller order
+  uint32_t n, n_tiles;             // jobs; tiles of CORDUM_SUBSET_TILE over them
+  uint32_t w_arg, w_rule, passes;  // key field widths; 8-bit radix passes = ceil(key bits / 8)
+  // scratch (device)
+  unsigned long long* keys[2];     // [n] each: pass p reads keys[p & 1], writes keys[(p + 1) & 1]
+  uint32_t* vals[2];               // [n] each: job indices alongside
+  uint32_t *counts, *totals;       // [256][n_tiles], [256]
+  uint32_t* jflag;                 // [n] job space: 1 = first job of its class, then its rank among the tile's first jobs
+  uint32_t* sloc;                  // [n] sorted space: class boundaries before the position within its tile
+  uint32_t *hcnt, *jcnt, *ccnt;    // [n_tiles] each: boundaries, first jobs, class sizes per tile; prefixes after the scans
+  uint32_t* head;                  // [2]: classes, record-check flag (a field wider than its key width); zeroed by the host
+  uint32_t *perm, *start, *size;   // [n] each: sorted-order class -> class; per class: first sorted position, its jobs (then
+                                   // its offset inside its tile of classes)
+  // output (device)
+  cordum_response_class* cls;      // [n] (classes in first_job order)
+  uint32_t* offsets;               // [n + 1]
+  uint32_t* jobs;                  // [n]
+};
+// key -> passes x (count, scan, scatter) -> heads -> ranks -> tile scan -> classes -> class scan -> tile scan -> gather
+cudaError_t launch_responses(const RespParams& P, cudaStream_t s);
+inline uint32_t responses_launches(const RespParams& P) { return P.n ? 8u + 3u * P.passes : 0u; }
+
 // ---- device-side encoder (encode.cu)
 struct EncodeParams {
   uint32_t n_jobs;

@@ -156,6 +156,29 @@ class Batch:
                                count=n * wire.COUNT_COLUMNS).reshape(n, wire.COUNT_COLUMNS)
         return labels, counts
 
+    def responses(self, flavor: int = wire.REASON_FLAVOR_KERNEL) -> dict:
+        """The last completed dispatch's jobs grouped by safety response class (cordum_batch_responses): {"classes":
+        wire.RESPONSE_CLASS_DTYPE [m] in first_job order, "reasons": [str] and "rule_ids": [str] per class, "offsets":
+        uint32 [m + 1], "jobs": uint32 [n] (class c holds jobs[offsets[c]:offsets[c+1]], ascending), "policy_gen": int}.
+        The arrays are views of library memory, valid until this batch's next encode, dispatch, responses call or free."""
+        r = wire.CordumResponses()
+        self.eng._ck(self.L.cordum_batch_responses(self.h, flavor, C.byref(r)))
+        m, n = r.n_classes, r.n_jobs
+
+        def view(ptr, count, dtype=np.uint32):
+            if not count:
+                return np.zeros(0, dtype)
+            return np.frombuffer((C.c_uint8 * (count * np.dtype(dtype).itemsize)).from_address(ptr), dtype=dtype, count=count)
+
+        def texts(off_ptr, bytes_ptr):
+            off = view(off_ptr, m + 1)
+            raw = C.string_at(bytes_ptr, int(off[m])) if off[m] else b""
+            return [raw[off[c]:off[c + 1]].decode("utf-8", "replace") for c in range(m)]
+
+        return {"classes": view(r.classes, m, wire.RESPONSE_CLASS_DTYPE), "reasons": texts(r.reason_off, r.reason_bytes),
+                "rule_ids": texts(r.rule_id_off, r.rule_id_bytes), "offsets": view(r.offsets, m + 1), "jobs": view(r.jobs, n),
+                "policy_gen": int(r.policy_gen)}
+
     def subset(self, dst: "Batch", outcomes: int = None, jobs=None) -> int:
         """Make `dst` the encoded batch of a subset of this one (cordum_batch_subset), on the device: the jobs whose plan
         outcome bucket k has bit k set in `outcomes` (e.g. wire.SUBSET_RETRYABLE), or the strictly ascending job indices

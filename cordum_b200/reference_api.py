@@ -13,6 +13,7 @@ tests read like the reference's own:
   MemoryRegistry.{update_heartbeat,snapshot} scheduler.MemoryRegistry              registry_memory.go:11-84
   Scheduler.process_jobs                     Engine.processJob's decision switch   engine.go:294-347,393
   topic_metrics(labels, counts)              the four topic-labelled counters      metrics/metrics.go:48-70
+  decision_records(batch, engine)            checkSafetyDecision's stored records  engine.go:524-545, emitDLQ :325-346
 
 Requests are plain dicts shaped like the CAP v2 messages (SURVEY App. B).  Every decision and
 every routed subject comes from the GPU (cordum_dispatch); this module only maps fields,
@@ -368,6 +369,37 @@ class Scheduler:
                         "rule_id": self.engine.rule_id(int(rec["rule_idx"])) if rec["rule_idx"] >= 0 else "",
                         "approval_required": bool(rec["flags"] & wire.F_APPROVAL_REQUIRED), "subject": subject, "error": err})
         return out
+
+
+def decision_records(batch, engine: Engine, flavor: int = wire.REASON_FLAVOR_KERNEL) -> list[dict]:
+    """What checkSafetyDecision stores for the jobs of each response class of Batch.responses() (engine.go:524-545), and
+    the reason code emitDLQ files a dead-lettered job under (engine.go:325-346): one dict per class, in the classes'
+    first_job order, with "jobs" (its job indices), "record" (the SafetyDecisionRecord fields SafetyClient.Check fills,
+    safety_client.go:104-113, as the job store keeps them, job_store.go:1036-1093) and "dlq_reason_code" (None for a job
+    that is not dead-lettered).  Constraints and remediations are looked up once per class, from the policy generation
+    the batch ran under."""
+    resp = batch.responses(flavor)
+    snapshot = batch.snapshot()
+    gen = resp["policy_gen"]
+    offsets, jobs = resp["offsets"], resp["jobs"]
+    out = []
+    for c, k in enumerate(resp["classes"]):
+        flags, rule_idx, sched = int(k["flags"]), int(k["rule_idx"]), int(k["sched_decision"])
+        record = {
+            # decisionFromProto (safety_client.go:105, :117-132), then the approval post-step (engine.go:527-529)
+            "decision": SAFETY_DECISION.get(sched, "DENY"),
+            "reason": resp["reasons"][c],                                                                  # safety_client.go:106
+            "rule_id": resp["rule_ids"][c],                                                                # safety_client.go:107
+            "policy_snapshot": snapshot if flags & wire.F_HAS_SNAPSHOT else "",                            # safety_client.go:108
+            "constraints": engine.rule_constraints(rule_idx, gen) if flags & wire.F_CONSTRAINTS else None,  # safety_client.go:109
+            "approval_required": bool(flags & wire.F_APPROVAL_REQUIRED),                                   # safety_client.go:110
+            "remediations": engine.rule_remediations(rule_idx, gen) if rule_idx >= 0 else [],             # safety_client.go:112
+        }
+        # emitDLQ: DENY -> "safety_denied" (engine.go:335), the default branch (an unknown decision) -> "safety_unknown"
+        # (engine.go:345); every other decision is not dead-lettered here
+        dlq = "safety_denied" if sched == wire.DEC_DENY else "safety_unknown" if sched == wire.DEC_UNSPECIFIED else None
+        out.append({"jobs": jobs[offsets[c]:offsets[c + 1]].copy(), "record": record, "dlq_reason_code": dlq})
+    return out
 
 
 JOB_STATUS_FAILED = "JOB_STATUS_FAILED"   # pb.JobStatus_JOB_STATUS_FAILED.String()

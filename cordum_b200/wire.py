@@ -130,6 +130,20 @@ class CordumTopicCounts(C.Structure):
                 ("counts", C.c_void_p)]
 
 
+class CordumResponses(C.Structure):
+    """cordum_responses: a dispatched batch's jobs grouped by safety response class, one reason and rule id per class
+    (cordum_batch_responses)."""
+    _fields_ = [("n_classes", C.c_uint32), ("n_jobs", C.c_uint32), ("policy_gen", C.c_uint64), ("classes", C.c_void_p),
+                ("offsets", C.c_void_p), ("jobs", C.c_void_p), ("reason_off", C.c_void_p), ("reason_bytes", C.c_void_p),
+                ("rule_id_off", C.c_void_p), ("rule_id_bytes", C.c_void_p)]
+
+
+# cordum_response_class (16 B)
+RESPONSE_CLASS_DTYPE = np.dtype([("decision", "u1"), ("sched_decision", "u1"), ("flags", "u1"), ("reason_code", "u1"),
+                                 ("rule_idx", "<i4"), ("arg", "<u4"), ("first_job", "<u4")])
+assert RESPONSE_CLASS_DTYPE.itemsize == 16
+
+
 class CordumEnvelopeCaps(C.Structure):
     _fields_ = [("max_jobs", C.c_uint32), ("max_risk_tags", C.c_uint32), ("max_requires", C.c_uint32), ("max_labels", C.c_uint32),
                 ("arena_bytes", C.c_uint64)]
@@ -167,6 +181,9 @@ COUNT_ROUTED = PLAN_OUTCOMES
 COUNT_COLUMNS = PLAN_OUTCOMES + 1
 REASON_NONE, REASON_RULE, REASON_MISSING_TOPIC, REASON_UNSUPPORTED_TOPIC, REASON_TENANT_MCP = 0, 1, 2, 3, 4
 REASON_EFF_DENIED_TOPIC, REASON_EFF_NOT_ALLOWED_TOPIC, REASON_EFF_MCP, REASON_APPROVAL_GRANTED = 12, 13, 14, 22
+# batch responses: the class key's flag mask, and the class flag of a reason that quotes an MCP value (canonical spelling)
+CLASS_FLAG_MASK = F_APPROVAL_REQUIRED | F_HAS_SNAPSHOT | F_CONSTRAINTS | F_APPROVED_BYPASS
+CLASS_QUOTES_VALUE = 0x80
 
 
 def _ptr(a: np.ndarray | None):

@@ -481,6 +481,57 @@ typedef struct cordum_topic_counts {
 } cordum_topic_counts;
 int32_t cordum_batch_topic_counts(cordum_batch* b, cordum_topic_counts* out);
 
+/* ---- batch responses: a dispatched batch's jobs grouped by the safety response checkSafetyDecision stores for them
+ * (SafetyDecisionRecord, engine.go:524-545, job_store.go:1036-1093: decision, reason, rule_id, policy_snapshot,
+ * constraints, remediations, approval_required), with each group's reason and rule id rendered once.  emitDLQ needs the
+ * reason of every denied job (engine.go:325-346) and the throttle path puts it into its retry message (:303-315); a bulk
+ * caller gets them here without a string build per job.
+ *
+ * Class key: two jobs share a class exactly when they agree on decision, sched_decision, flags & (APPROVAL_REQUIRED |
+ * HAS_SNAPSHOT | CONSTRAINTS | APPROVED_BYPASS) (F_TIE and every route field are left out), reason_code, rule_idx and arg:
+ * the job's topic id for EFF_DENIED_TOPIC / EFF_NOT_ALLOWED_TOPIC, its MCP value id of field k >> 1 for TENANT_MCP + k /
+ * EFF_MCP + k, 0 for every other code.  Classes are distinct keys, not distinct texts: two raw topics that trim to the same
+ * text are two classes with equal reasons.
+ * Rendered per class, equal to what the front-end builds for each member job (frontend.cpp):
+ *   reason:  "" for ALLOW / ALLOW_WITH_CONSTRAINTS unless the code is APPROVAL_GRANTED (kernel.go:198-215); otherwise
+ *            cordum_reason_flavor(e, b, first_job, flavor, NULL, ...).  An MCP reason quotes the canonical (case-folded)
+ *            spelling of the value and its class carries CORDUM_CLASS_QUOTES_VALUE; a value that no MCP list names has
+ *            no dictionary spelling (all such values share one id and one class per field and code) and is quoted as "".
+ *            A caller that still holds the envelopes and wants the request's own spelling calls cordum_reason_flavor
+ *            with them for the jobs of those classes only.
+ *   rule_id: rules[rule_idx].id of the batch's policy generation when HAS_SNAPSHOT is set, else "".
+ * Constraints and remediations are not copied: cordum_rule_*_json_at(policy_gen, rule_idx) once per distinct rule.  Both
+ * flavours have the same partition.
+ * Valid exactly when cordum_batch_plan is (subset and merge destinations once dispatched, a device encode that fell back to
+ * the host encoder included); otherwise CORDUM_E_STATE.  CORDUM_E_INVALID for NULL arguments or flavor > 1, CORDUM_E_CUDA on
+ * a failed engine, CORDUM_E_STALE when a class has an MCP reason code and the batch's table epoch has passed (the value
+ * dictionaries were rebuilt: cordum_reason returns -1 for those jobs too); rule and topic text come from the batch's own
+ * generation, so a batch without MCP classes keeps working across reloads.  CORDUM_E_CAPACITY when the key does not fit
+ * 64 bits or the scratch does not fit; the engine stays usable.
+ * Synchronous.  The arrays are pinned memory owned by the batch, valid until its next encode, dispatch, responses call or
+ * free; the plan, the topic counts and the responses use separate buffers.  Only the class descriptors, the offsets and the
+ * job list cross PCIe; the host renders one reason and one rule id per class.  Kernel launches, counted by
+ * cordum_launch_count: 8 + 3 x ceil(key bits / 8), key bits = 15 + bits(n_rules + 1) + max(16, bits(topic ids of the
+ * batch's dictionary generation)); 0 for an empty batch.  NVTX range "cordum:responses". */
+typedef struct cordum_response_class {
+  uint8_t decision, sched_decision, flags, reason_code; /* as in cordum_decision; flags masked as in the key, plus
+                                                           CORDUM_CLASS_QUOTES_VALUE                                  */
+  int32_t rule_idx;                                     /* -1 = none                                                  */
+  uint32_t arg;                                         /* topic id or MCP value id, see the key; 0 when unused       */
+  uint32_t first_job;                                   /* lowest original job index in the class                     */
+} cordum_response_class;                                /* 16 B */
+typedef struct cordum_responses {
+  uint32_t n_classes, n_jobs;
+  uint64_t policy_gen;                     /* = cordum_batch_policy_gen(b): for cordum_rule_*_json_at                */
+  const cordum_response_class* classes;    /* [n_classes], ordered by first_job ascending                            */
+  const uint32_t* offsets;                 /* [n_classes + 1]: class c holds jobs[offsets[c] .. offsets[c+1])        */
+  const uint32_t* jobs;                    /* [n_jobs] original job indices, ascending inside a class                */
+  const uint32_t* reason_off;  const uint8_t* reason_bytes;   /* [n_classes + 1] + arena: the response's Reason      */
+  const uint32_t* rule_id_off; const uint8_t* rule_id_bytes;  /* [n_classes + 1] + arena: the response's RuleId      */
+} cordum_responses;
+#define CORDUM_CLASS_QUOTES_VALUE 0x80   /* in classes[c].flags: the reason quotes an MCP value (canonical spelling) */
+int32_t cordum_batch_responses(cordum_batch* b, uint32_t flavor, cordum_responses* out);
+
 /* Host-side materialisation of what the record indexes (pure functions of rule_idx /
  * reason_code / worker_slot; SURVEY.md A.5).  Each writes a NUL-terminated string
  * into buf (truncating to cap) and returns the full length. */

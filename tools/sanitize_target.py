@@ -1,6 +1,6 @@
 """Small end-to-end run of every kernel for compute-sanitizer (tools/sanitize.sh): policy_kernel, route_kernel (label
 picks, multi-chunk and unsorted pools), worker_chunk / worker_merge, the device encoder, heartbeat ingest, scheduler ticks,
-the wide-mask path, the dispatch plan kernels, the batch subset and merge kernels and the topic count kernels.  Checks the
+the wide-mask path, the dispatch plan kernels, the batch subset and merge kernels, the topic count kernels and the response kernels.  Checks the
 results against the oracle (the plan against a numpy grouping of the records, a subset against its source's records, a
 merge against a host encode of both sources' envelopes and their records, the topic counts against the records grouped
 by trimmed topic), so a sanitizer-clean run is also a correct one."""
@@ -55,6 +55,22 @@ def counts_same(b, rec, topics, what):
 def topics_of(env):
     t = env.cols["topic"][:env.n_jobs]
     return [bytes(env.arena[int(o):int(o) + int(n)]) for o, n in zip(t["off"], t["len"])]
+
+
+def responses_same(b, rec, what):
+    """Batch.responses(): every job once, jobs ascending inside a class, classes by first job, each class one key of the
+    records (masked flags, reason code, rule index) and each job's reason the library's per-job one."""
+    resp = b.responses()
+    off, jobs, cls = resp["offsets"].astype(np.int64), resp["jobs"].astype(np.int64), resp["classes"]
+    assert off[-1] == len(rec) and np.array_equal(np.sort(jobs), np.arange(len(rec))), what
+    assert (np.diff(cls["first_job"].astype(np.int64)) > 0).all(), what
+    for c in range(len(cls)):
+        m = jobs[off[c]:off[c + 1]]
+        assert m[0] == cls["first_job"][c] and (np.diff(m) > 0).all(), what
+        r = rec[m]
+        assert (r["reason_code"] == cls["reason_code"][c]).all() and (r["rule_idx"] == cls["rule_idx"][c]).all(), what
+        assert ((r["flags"] & wire.CLASS_FLAG_MASK) == (cls["flags"][c] & wire.CLASS_FLAG_MASK)).all(), what
+    print("ok: responses,", what, len(cls), "classes", flush=True)
 
 
 def subset_same(b, dst, rec, what):
@@ -132,6 +148,7 @@ def main():
                [{"topic": "job.w.go", "labels": {"host": "m%05d" % (i % 97), "zone": "z%d" % (i % 4)}} for i in range(64)] + [{"topic": "job.w.go"}] * 8
         same(b.encode(jobs).dispatch(wire.MODE_ROUTE_ONLY), o2.eval(jobs, wire.MODE_ROUTE_ONLY), "pool of %d workers" % size)
         plan_same(b, b.results(), size, "pool of %d workers" % size)
+        responses_same(b, b.results(), "pool of %d workers" % size)
         o2.close()
     # wide masks
     sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -144,6 +161,7 @@ def main():
     o3 = oracle_lib.Oracle(policy, routing, workers)
     bw = e.batch(len(jobs))
     same(bw.encode(jobs).dispatch(), o3.eval(jobs), "wide masks")
+    responses_same(bw, bw.results(), "wide masks")
     subset_same(bw, e.batch(len(jobs)), bw.results().copy(), "wide masks")
     merge_same(e, bw, jobs, "wide masks")
     o3.close()
@@ -178,6 +196,7 @@ def main():
     o4.update_workers(np.arange(W, dtype=np.uint32), keep[3])
     same(b2.fetch(), o4.eval(cfg.jobs), "ticks")
     plan_same(b2, b2.results(), W, "ticks")
+    responses_same(b2, b2.results(), "ticks")
     o4.close()
     o.close()
     print("sanitize target done", flush=True)
